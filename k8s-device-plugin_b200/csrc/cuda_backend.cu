@@ -37,13 +37,7 @@
 
 namespace b2dp {
 
-// ---- kernel shapes chosen with tools/probe_sweep on an H100 SXM (80 GB HBM3, 700 W) ----------------------------
-constexpr int kTmaCW = 4;           // verifier warps
-constexpr int kTmaTileVec = 1024;   // 16 KiB tiles
-constexpr int kTmaStages = 3;
-constexpr int kTmaCtasPerSm = 2;    // 2 x 3 x 16 KiB = 96 KiB staged per SM
-constexpr size_t kTmaSmem = (size_t)kTmaStages * kTmaTileVec * 16 + 2 * kTmaStages * 8;
-constexpr int kRegThreads = 512, kRegUnroll = 2, kRegCtasPerSm = 2;
+// the kernel shapes (kTma*, kReg*) are defined next to the kernels in hbm_probe.cuh
 constexpr unsigned long long kFloorMinBytes = 128ull << 20;  // a ring slot well above the 50 MB L2: the pass measures HBM, not the cache
 
 // bit b of (uint32(i) * K) summed over i < n_words, for the closed-form checksum

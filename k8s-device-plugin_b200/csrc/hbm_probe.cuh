@@ -22,12 +22,24 @@
 // (~25 KB to cover HBM latency at 3.35 TB/s / 132 SMs) and a grid that is a
 // multiple of the SM count.
 #pragma once
+#include <cstddef>
 #include <cstdint>
 #include <cuda_runtime.h>
 
 namespace b2dp {
 
 constexpr uint32_t kPatternMul = 2654435761u;
+
+// Dynamic shared memory of one hbm_probe_tma CTA: the tile ring plus its full/done mbarriers.
+constexpr size_t tma_smem_bytes(int tile_vec, int stages) { return (size_t)stages * tile_vec * 16 + 2 * stages * 8; }
+
+// ---- the product's kernel shapes, chosen with tools/probe_sweep on an H100 SXM (80 GB HBM3, 700 W) ----------------
+constexpr int kTmaCW = 4;           // verifier warps
+constexpr int kTmaTileVec = 1024;   // 16 KiB tiles
+constexpr int kTmaStages = 3;
+constexpr int kTmaCtasPerSm = 2;    // 2 x 3 x 16 KiB = 96 KiB staged per SM
+constexpr size_t kTmaSmem = tma_smem_bytes(kTmaTileVec, kTmaStages);
+constexpr int kRegThreads = 512, kRegUnroll = 2, kRegCtasPerSm = 2;
 
 // Device-resident control block (one per GPU, zero-initialised once).
 struct ProbeCtl {

@@ -80,6 +80,94 @@ def test_fault_injection_flips_health(P, variant):
         assert [d.health for d in P.v1beta1.ListAndWatchResponse.FromString(wire).devices] == ["Healthy"]
 
 
+@pytest.mark.parametrize("variant", [0, 1])
+@pytest.mark.parametrize("nbytes", [MiB + 48, 3 * MiB + 16 * 37])
+def test_grid_ctas_bit_exact(P, nbytes, variant):
+    """`grid_ctas` from one CTA (every tile and the whole ragged tail on one CTA) to more CTAs than tiles: buffer
+    contents and every result field equal the oracle, pass after pass on the same ring."""
+    n_words = nbytes // 4
+    with _open(P, nbytes) as ctx:
+        seed = oprobe.initial_seed(0)
+        for grid in (1, 2, 7, 131, 264, 1000):
+            before = ctx.probe_peek(0, 0, n_words)
+            assert np.array_equal(before, oprobe.pattern(n_words, seed)), grid
+            (r,) = ctx.probe_health(variant=variant, min_gbs=1e-3, grid_ctas=grid)
+            cs, bad, first, dst = oprobe.probe_pass(before, seed, oprobe.next_seed(seed))
+            assert r.err == 0 and r.seed == seed and r.bytes == 2 * nbytes, grid
+            assert (r.checksum, r.mismatches, r.first_bad_word) == (cs, bad, first) == (cs, 0, oprobe.NO_BAD), grid
+            assert r.checksum == r.expected_checksum and r.healthy, grid
+            assert np.array_equal(ctx.probe_peek(0, 0, n_words), dst), grid
+            seed = oprobe.next_seed(seed)
+
+
+@pytest.mark.parametrize("variant", [0, 1])
+def test_dense_injected_faults_equal_oracle(P, variant):
+    """48 corrupted words: all four lanes of one vector, both sides of several 16 KiB tile (chunk) boundaries, the
+    ragged tail and the last word.  Every result field equals the oracle on the corrupted source; the fault is
+    reported once and the next pass is clean."""
+    nbytes = 8 * MiB + 16 * 5
+    n_words = nbytes // 4
+    tile = 4 * 1024                                   # words per TMA tile and per R128 chunk
+    words = {4 * 777 + lane for lane in range(4)}
+    for t in (1, 2, 263, 264, 511):
+        words |= {t * tile - 1, t * tile}
+    words |= {(n_words // tile) * tile, n_words - 17, n_words - 2, n_words - 1}
+    rng = np.random.default_rng(48)
+    while len(words) < 48:
+        words.add(int(rng.integers(0, n_words)))
+    words = sorted(words)
+    masks = [int(m) for m in rng.integers(1, 1 << 32, len(words), dtype=np.uint64)]
+    with _open(P, nbytes) as ctx:
+        seed = oprobe.initial_seed(0)
+        for w, m in zip(words, masks):
+            ctx.probe_inject_fault(0, w, m)
+        src = ctx.probe_peek(0, 0, n_words)
+        cs, bad, first, _ = oprobe.probe_pass(src, seed, oprobe.next_seed(seed))
+        (r,) = ctx.probe_health(variant=variant, min_gbs=1e-3)
+        assert (r.checksum, r.mismatches, r.first_bad_word) == (cs, bad, first) == (cs, 48, words[0])
+        assert r.seed == seed and not r.healthy
+        seed = oprobe.next_seed(seed)
+        assert np.array_equal(ctx.probe_peek(0, 0, n_words), oprobe.pattern(n_words, seed))
+        (r,) = ctx.probe_health(variant=variant, min_gbs=1e-3)
+        assert r.healthy and r.mismatches == 0 and r.first_bad_word == oprobe.NO_BAD
+
+
+def _sum_preserving_pair(seed, n_words, bit, lo=0):
+    """Two word indices >= lo whose pattern(seed) words have `bit` clear and set: flipping that bit in both keeps the
+    sum of the buffer."""
+    pat = oprobe.pattern(n_words - lo, seed, lo)
+    b = (pat >> np.uint32(bit)) & np.uint32(1)
+    i = lo + int(np.nonzero(b == 0)[0][0])
+    j = lo + int(np.nonzero(b == 1)[0][-1])
+    return i, j
+
+
+@pytest.mark.parametrize("variant", [0, 1])
+def test_checksum_preserving_pair_fails_the_device(P, variant):
+    """Bit b flipped 0->1 in one word and 1->0 in another leaves the checksum equal to the closed form: only the
+    mismatch count can fail the device, and it must."""
+    nbytes = 4 * MiB + 16 * 3
+    n_words = nbytes // 4
+    with _open(P, nbytes) as ctx:
+        seed = oprobe.initial_seed(0)
+        i, j = _sum_preserving_pair(seed, n_words, 13, lo=1000)
+        ctx.probe_inject_fault(0, i, 1 << 13)
+        ctx.probe_inject_fault(0, j, 1 << 13)
+        (r,) = ctx.probe_health(variant=variant, min_gbs=1e-3)
+        assert r.checksum == r.expected_checksum == oprobe.expected_checksum(n_words, seed)
+        assert (r.mismatches, r.first_bad_word, r.healthy) == (2, min(i, j), 0)
+        # through the kubelet-facing heartbeat (the library re-filled the ring after reporting)
+        seed = oprobe.next_seed(seed)
+        i, j = _sum_preserving_pair(seed, n_words, 31)
+        ctx.probe_inject_fault(0, i, 1 << 31)
+        ctx.probe_inject_fault(0, j, 1 << 31)
+        wire, st = ctx.list_and_watch("gpu", P._native.LW_HEARTBEAT, variant=variant, min_gbs=1e-3)
+        assert [d.health for d in P.v1beta1.ListAndWatchResponse.FromString(wire).devices] == ["Unhealthy"]
+        assert st.n_unhealthy == 1
+        wire, st = ctx.list_and_watch("gpu", P._native.LW_HEARTBEAT, variant=variant, min_gbs=1e-3)
+        assert [d.health for d in P.v1beta1.ListAndWatchResponse.FromString(wire).devices] == ["Healthy"]
+
+
 def _driver_copy_gbs(nbytes):
     """Best of 10 CUDA-event-timed torch device-to-device copies of nbytes: GB/s read + written."""
     import torch
@@ -274,6 +362,52 @@ def test_p2p_matrix(P):
         assert ctx.generate_labels(["p2p-link"]) == {
             "amd.com/gpu.p2p-link": cls, "beta.amd.com/gpu.p2p-link": cls, "beta.amd.com/gpu.p2p-link." + cls: str(n)}
         assert P.labeller.removeOldNodeLabels(ctx.generate_labels(["p2p-link", "vram"])) == {}
+
+
+def test_p2p_matrix_detects_a_corrupt_peer(P):
+    """A P2P pass is a verify-only pass (delta 0) over the peer's current slot: a flipped word, and a checksum-
+    preserving pair, in GPU j's slot show up as mism[i][j] for every reader i with peer access and nowhere else.  The
+    matrix reads only the first p2p_bytes, so a fault past them is left for j's own next probe, which reports it once."""
+    import torch
+    if torch.cuda.device_count() < 2:
+        pytest.skip("the P2P matrix needs 2 or more GPUs; this node has %d" % torch.cuda.device_count())
+    nbytes, p2p_bytes = 64 * MiB, 16 * MiB
+    with P.Context("cuda:bytes=%d,p2p_bytes=%d" % (nbytes, p2p_bytes)) as ctx:
+        n = len(ctx.enumerate())
+        j = n - 1
+        _, lt, mm = ctx.p2p_matrix()
+        assert (mm == 0).all()
+        readers = [i for i in range(n) if i != j and lt[i, j] != 0]     # link type 0 off the diagonal: no peer access
+        assert readers, lt
+
+        def expect(count):
+            want = np.zeros((n, n), dtype=mm.dtype)
+            want[readers, j] = count
+            return want
+
+        ctx.probe_inject_fault(j, 12345, 0x10)
+        _, _, mm = ctx.p2p_matrix()
+        assert (mm == expect(1)).all(), mm
+        res = ctx.probe_health(min_gbs=1e-3)                            # the matrix left j's slot as it was
+        assert [(r.mismatches, r.first_bad_word) for r in res if r.device == j] == [(1, 12345)]
+        assert all(r.healthy for r in res if r.device != j)
+
+        seed = oprobe.next_seed([r.seed for r in res if r.device == j][0])   # j's slot was re-filled for the next pass
+        a, b = _sum_preserving_pair(seed, 1 << 16, 7)
+        ctx.probe_inject_fault(j, a, 1 << 7)
+        ctx.probe_inject_fault(j, b, 1 << 7)
+        _, _, mm = ctx.p2p_matrix()
+        assert (mm == expect(2)).all(), mm
+        res = ctx.probe_health(min_gbs=1e-3)
+        assert [(r.mismatches, r.checksum == r.expected_checksum) for r in res if r.device == j] == [(2, True)]
+
+        past = p2p_bytes // 4 + 100
+        ctx.probe_inject_fault(j, past, 0x1)
+        _, _, mm = ctx.p2p_matrix()
+        assert (mm == 0).all(), mm
+        res = ctx.probe_health(min_gbs=1e-3)
+        assert [(r.mismatches, r.first_bad_word) for r in res if r.device == j] == [(1, past)]
+        assert all(r.healthy for r in ctx.probe_health(min_gbs=1e-3))
 
 
 def test_multi_gpu_fanout_concurrent(P):
