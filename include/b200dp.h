@@ -268,6 +268,8 @@ typedef struct b2dp_probe_result {
                                       heartbeat only rang the doorbell (no launch on its critical path) */
 #define B2DP_RES_XID 0x8u          /* xid=1: a critical Xid event was delivered for this device since open (or the
                                       last b2dp_probe_reset) => Unhealthy, sticky */
+#define B2DP_RES_MEMTEST 0x200u    /* a b2dp_memtest of this device failed or timed out since open (or the last
+                                      b2dp_probe_reset) => Unhealthy, sticky */
 
 /* Replaces the exporter round trip getGPUHealth (exporter/health.go:42-82) and the evidence behind simpleHealthCheck
  * (plugin.go:161-206): launch the probe on every GPU of the context concurrently (one worker thread + stream per
@@ -278,7 +280,8 @@ B2DP_API int b2dp_probe_health(b2dp_ctx *ctx, const b2dp_probe_opts *opts, b2dp_
  * NEXT probe of `device` will read.  word_index == UINT64_MAX instead queues a synthetic critical-Xid
  * event numbered `mask` for `device` (seen by contexts opened with xid=1).  The reference has no equivalent. */
 B2DP_API int b2dp_probe_inject_fault(b2dp_ctx *ctx, int device, uint64_t word_index, uint32_t mask);
-/* Re-fill the probe buffers of `device` (-1 = all) with a clean pattern; also clears a latched Xid. */
+/* Re-fill the probe buffers of `device` (-1 = all) with a clean pattern; also clears a latched Xid and a latched memtest
+ * failure. */
 B2DP_API int b2dp_probe_reset(b2dp_ctx *ctx, int device);
 /* Set the bandwidth ceiling (gbs_ref) of `device` (-1 = all) the fractional floor refers to, e.g. to the site's measured
  * HBM peak; gbs_ref <= 0 restores the device's own calibration.  Also how tests move a device across the 0.8 line. */
@@ -304,6 +307,56 @@ B2DP_API int b2dp_expected_checksum(uint64_t n_words, uint32_t seed, uint64_t *c
 /* Copy `n_words` words starting at `word_index` of the buffer the next probe will read
  * (parity tests compare it with the oracle's pattern). */
 B2DP_API int b2dp_probe_peek(b2dp_ctx *ctx, int device, uint64_t word_index, uint32_t *out, uint64_t n_words);
+
+/* ---- on-demand memory test (feeds the same per-GPU verdict as the probe) ------------ */
+typedef struct b2dp_memtest_opts {
+    uint64_t max_bytes;      /* cap on the bytes tested per device; 0 = all free memory above the reserve */
+    uint64_t reserve_bytes;  /* memory left free for others; 0 = 10 % of the device's total memory */
+    uint32_t timeout_ms;     /* per-call deadline; 0 = 60000 */
+    uint32_t flags;          /* B2DP_MT_EVEN_IF_BUSY */
+    uint64_t fault_word;     /* test hook: XOR fault_mask into this word of the tested span (global word index over the
+                                segments) right after the first march element; ignored when fault_mask = 0 */
+    uint32_t fault_mask;
+    uint32_t reserved;
+} b2dp_memtest_opts;
+#define B2DP_MT_EVEN_IF_BUSY 0x1u  /* test a GPU even while another process uses it (default: skip it) */
+
+typedef struct b2dp_memtest_result {
+    int32_t device;             /* index into b2dp_enumerate() order */
+    int32_t healthy;            /* 1 Healthy, 0 Unhealthy (a failure is latched: B2DP_RES_MEMTEST) */
+    int32_t err;                /* B2DP_OK | B2DP_E_CUDA | B2DP_E_TIMEOUT | B2DP_E_INVAL (fault_word outside the span) */
+    uint32_t flags;             /* B2DP_MT_* */
+    uint32_t seed;              /* pattern seed of the test; segment g is keyed with seed ^ uint32(g * 0x9E3779B9) */
+    int32_t n_segments;         /* allocations the tested span is made of (1 GiB each, the last may be smaller) */
+    uint64_t bytes_tested;
+    uint64_t free_before;       /* free device memory before the test (cudaMemGetInfo) */
+    uint64_t total_memory;
+    uint64_t mismatches[4];     /* per march element: E0 w(P) (always 0), E1 r(P) w(~P), E2 r(~P) w(P), E3 r(P) */
+    uint64_t first_bad_word;    /* min bad global word index over the elements, UINT64_MAX if none */
+    uint64_t ecc_corrected;     /* NVML volatile ECC deltas over the test (0 without NVML: B2DP_MT_NO_ECC) */
+    uint64_t ecc_uncorrected;
+    float ms;                   /* CUDA-event time of the four elements */
+    float gbs;                  /* algorithmic traffic 6 * bytes_tested / ms */
+} b2dp_memtest_result;
+#define B2DP_MT_SKIPPED_BUSY 0x1u   /* another process uses the GPU: nothing allocated, nothing tested, nothing latched;
+                                       healthy = the last heartbeat verdict */
+#define B2DP_MT_PARTIAL 0x2u        /* an allocation failed part way (memory taken meanwhile): the part obtained was tested */
+#define B2DP_MT_ECC_CORRECTED 0x4u  /* corrected ECC errors appeared during the test (reported, not failed) */
+#define B2DP_MT_ECC 0x8u            /* uncorrected ECC errors appeared, or a row remap failed or is pending => Unhealthy */
+#define B2DP_MT_NO_ECC 0x10u        /* NVML could not report ECC counters: the verdict rests on the data alone */
+#define B2DP_MT_EMPTY 0x20u         /* no memory above the reserve: nothing was tested (not a verdict on the part) */
+
+/* An on-demand test of the free HBM of `device` (-1 = every GPU, concurrently on their workers): the evidence behind
+ * the per-GPU verdict the exporter round trip supplies in the reference (exporter/health.go:42-82), merged the same
+ * way (exporter/health.go:86-106) through the sticky B2DP_RES_MEMTEST bit.  Per GPU: sizes the test from free memory
+ * (cudaMemGetInfo, reserve, max_bytes), allocates it in <= 1 GiB segments, runs the 4-element march in place
+ * (hbm_memtest.cuh), reads the NVML ECC / row-remap counters around it and frees every segment before the call
+ * returns, on every path (a device that misses the deadline is reported B2DP_E_TIMEOUT, but the call still waits for
+ * its kernels, because memory a kernel uses cannot be released earlier).  The probe lock is held throughout: a
+ * heartbeat waits for a running memtest.  A GPU another process uses is skipped (B2DP_MT_SKIPPED_BUSY) unless
+ * B2DP_MT_EVEN_IF_BUSY.  cuda: backend with the in-process probe only; B2DP_E_UNSUPPORTED otherwise. */
+B2DP_API int b2dp_memtest(b2dp_ctx *ctx, int device, const b2dp_memtest_opts *opts, b2dp_memtest_result *out, int cap,
+                          int *n);
 
 /* exporter/health.go:86-106 PopulatePerGPUDHealth(devs, defaultHealth) merge rule.
  * have_source = 0 reproduces "exporter socket absent / RPC failed" (every device gets the

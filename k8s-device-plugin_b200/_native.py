@@ -38,6 +38,9 @@ PROBE_EVENT_TIMING = 0x20
 RES_SKIPPED_BUSY, RES_SHRUNK, RES_ECC, RES_XID, RES_SMALL_RING = 1, 2, 4, 8, 16
 RES_CONTENDED, RES_NO_FLOOR, RES_SLOW, RES_PREARMED = 0x20, 0x40, 0x80, 0x100
 LW_INITIAL, LW_HEARTBEAT, LW_EXTERNAL_SOURCE, LW_NO_PROBE, LW_LINK_CHECK = 1, 2, 4, 8, 16
+RES_MEMTEST = 0x200
+MT_EVEN_IF_BUSY = 1
+MT_SKIPPED_BUSY, MT_PARTIAL, MT_ECC_CORRECTED, MT_ECC, MT_NO_ECC, MT_EMPTY = 1, 2, 4, 8, 0x10, 0x20
 
 Id64 = C.c_char * 64
 
@@ -107,6 +110,18 @@ class P2pOpts(C.Structure):
     _fields_ = [("bytes", C.c_uint64), ("iters", C.c_uint32), ("flags", C.c_uint32)]
 
 
+class MemtestOpts(C.Structure):
+    _fields_ = [("max_bytes", C.c_uint64), ("reserve_bytes", C.c_uint64), ("timeout_ms", C.c_uint32), ("flags", C.c_uint32),
+                ("fault_word", C.c_uint64), ("fault_mask", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+class MemtestResult(C.Structure):
+    _fields_ = [("device", C.c_int32), ("healthy", C.c_int32), ("err", C.c_int32), ("flags", C.c_uint32),
+                ("seed", C.c_uint32), ("n_segments", C.c_int32), ("bytes_tested", C.c_uint64), ("free_before", C.c_uint64),
+                ("total_memory", C.c_uint64), ("mismatches", C.c_uint64 * 4), ("first_bad_word", C.c_uint64),
+                ("ecc_corrected", C.c_uint64), ("ecc_uncorrected", C.c_uint64), ("ms", C.c_float), ("gbs", C.c_float)]
+
+
 if not os.path.exists(LIB_PATH):
     raise ImportError(
         "libb200dp.so is not built: run `python -c 'import __graft_entry__ as g; g.build()'` "
@@ -145,6 +160,7 @@ SIGNATURES = {
     "b2dp_probe_inject_fault": (_i, [_vp, _i, C.c_uint64, C.c_uint32]),
     "b2dp_probe_reset": (_i, [_vp, _i]),
     "b2dp_probe_peek": (_i, [_vp, _i, C.c_uint64, _P(C.c_uint32), C.c_uint64]),
+    "b2dp_memtest": (_i, [_vp, _i, _P(MemtestOpts), _P(MemtestResult), _i, _ip]),
     "b2dp_probe_set_ref": (_i, [_vp, _i, C.c_float]),
     "b2dp_probe_describe": (_i, [_vp, _i, _P(ProbeInfo)]),
     "b2dp_expected_checksum": (_i, [C.c_uint64, C.c_uint32, _P(C.c_uint64)]),

@@ -28,6 +28,25 @@ class ProbeResult:
 
 
 @dataclass
+class MemtestResult:
+    device: int
+    healthy: bool
+    err: int
+    flags: int
+    seed: int
+    n_segments: int
+    bytes_tested: int
+    free_before: int
+    total_memory: int
+    mismatches: List[int]          # per march element: E0 w(P), E1 r(P) w(~P), E2 r(~P) w(P), E3 r(P)
+    first_bad_word: int
+    ecc_corrected: int
+    ecc_uncorrected: int
+    ms: float
+    gbs: float                     # 6 x bytes_tested / ms
+
+
+@dataclass
 class CycleStats:
     n_devices: int
     n_unhealthy: int
@@ -155,6 +174,21 @@ class Context:
         N.check(N.lib.b2dp_probe_peek(self._h, device, word_index, out.ctypes.data_as(C.POINTER(C.c_uint32)), n_words),
                 self._h)
         return out
+
+    def memtest(self, device: int = -1, max_bytes: int = 0, reserve_bytes: int = 0, timeout_ms: int = 0,
+                even_if_busy: bool = False, fault_word: int = 0, fault_mask: int = 0) -> List[MemtestResult]:
+        """On-demand march test of the free HBM of `device` (-1 = every GPU, b2dp_memtest).  max_bytes = 0 tests all
+        free memory above the reserve (reserve_bytes = 0: 10 % of the device's memory).  A failure is latched: later
+        probe results carry RES_MEMTEST and are Unhealthy until probe_reset().  fault_word / fault_mask is a test hook
+        that flips bits of the tested span after the first element."""
+        opts = N.MemtestOpts(max_bytes, reserve_bytes, timeout_ms, N.MT_EVEN_IF_BUSY if even_if_busy else 0, fault_word,
+                             fault_mask, 0)
+        rc, arr, n = N.grow_call(lambda cap: (N.MemtestResult * cap)(),
+                                 lambda a, cap, pn: N.lib.b2dp_memtest(self._h, device, C.byref(opts), a, cap, pn))
+        N.check(rc, self._h)
+        return [MemtestResult(r.device, bool(r.healthy), r.err, r.flags, r.seed, r.n_segments, r.bytes_tested,
+                              r.free_before, r.total_memory, list(r.mismatches), r.first_bad_word, r.ecc_corrected,
+                              r.ecc_uncorrected, r.ms, r.gbs) for r in arr[:n]]
 
     # ---- ListAndWatch --------------------------------------------------------------------
     def list_and_watch(self, resource: str = "gpu", flags: int = N.LW_INITIAL, external: Optional[Dict[str, bool]] = None,

@@ -52,6 +52,13 @@ struct b2dp_ctx {
 
 static int fail(int code, const std::string& msg) { t_last_error = msg; return code; }
 
+namespace b2dp {
+MemtestHooks& memtest_hooks() {
+    static MemtestHooks hooks;
+    return hooks;
+}
+}  // namespace b2dp
+
 static int enumerate_ctx(b2dp_ctx* c, std::vector<Device>& devs) {
     std::string err;
     int rc = c->kind == b2dp_ctx::KFD ? kfd_enumerate(c->sysroot, devs, err) : cuda_enumerate(c->cuda, devs, err);
@@ -432,6 +439,28 @@ extern "C" int b2dp_probe_peek(b2dp_ctx* c, int device, uint64_t word_index, uin
     return rc == B2DP_OK ? rc : fail(rc, err);
 }
 
+extern "C" int b2dp_memtest(b2dp_ctx* c, int device, const b2dp_memtest_opts* opts, b2dp_memtest_result* out, int cap,
+                            int* n) {
+    if (!c || !n || cap < 0) return B2DP_E_INVAL;
+    if (c->kind != b2dp_ctx::CUDA)
+        return fail(B2DP_E_UNSUPPORTED, "the memory test needs the cuda: backend (there is no CPU fallback)");
+    // the capacity is checked before the test runs: its results cannot be produced a second time for free
+    const int count = cuda_device_count(c->cuda);
+    if (device < -1 || device >= count) return fail(B2DP_E_INVAL, "device index out of range");
+    *n = device < 0 ? count : 1;
+    if (*n > cap) return B2DP_E_NOSPC;
+    if (*n && !out) return B2DP_E_INVAL;
+    std::vector<b2dp_memtest_result> res;
+    std::string err;
+    const MemtestHooks& mt = memtest_hooks();
+    if (!mt.run) return fail(B2DP_E_UNSUPPORTED, "this build of the library has no memory test");
+    int rc = mt.run(c->cuda, device, opts, res, err);
+    if (rc != B2DP_OK) return fail(rc, err);
+    *n = (int)res.size();
+    memcpy(out, res.data(), res.size() * sizeof(b2dp_memtest_result));
+    return B2DP_OK;
+}
+
 extern "C" int b2dp_merge_health(const char (*ids)[64], int n, int32_t default_healthy, int have_source,
                                  const char (*src_ids)[64], const int32_t* src_health, int m, int32_t* out) {
     if (n < 0 || m < 0 || (n && (!ids || !out)) || (have_source && m && (!src_ids || !src_health))) return B2DP_E_INVAL;
@@ -615,6 +644,10 @@ static void watch_send(b2dp_watch* w, uint32_t flags) {
 
 static void watch_loop(b2dp_watch* w) {
     watch_send(w, B2DP_LW_INITIAL);
+    // The initial list says every device is Healthy (plugin.go:231-299).  A device whose memory test has failed is
+    // reported by one heartbeat right away, so the kubelet learns of it even without a ticker (-pulse=0).
+    const MemtestHooks& mt = memtest_hooks();
+    if (w->ctx->kind == b2dp_ctx::CUDA && mt.latched && mt.latched(w->ctx->cuda)) watch_send(w, B2DP_LW_HEARTBEAT);
     auto next = std::chrono::steady_clock::now() + std::chrono::milliseconds(w->pulse_ms);
     for (;;) {
         {

@@ -29,8 +29,10 @@
 #include <thread>
 
 #include "gosem.hpp"
+#include "hbm_memtest.cuh"
 #include "hbm_probe.cuh"
 #include "internal.hpp"
+#include "memtest_math.hpp"
 #include "nvml_dyn.hpp"
 #include "pattern_math.hpp"
 #include "units_backend.hpp"
@@ -98,6 +100,7 @@ struct Gpu {
     bool have_ecc = false;
     bool xid_registered = false;
     std::atomic<unsigned long long> xid_fault{0};  // first critical Xid seen on this device (sticky, like a real fault)
+    std::atomic<bool> memtest_fault{false};        // a b2dp_memtest failed or timed out (sticky until b2dp_probe_reset)
     int last_healthy = 1;
     // worker
     std::thread th;
@@ -1101,6 +1104,12 @@ int cuda_probe(CudaBackend* be, const b2dp_probe_opts* opts, std::vector<b2dp_pr
                 be->gpus[i]->last_healthy = 0;
             }
     }
+    for (size_t i = 0; i < n; ++i)  // a failed memory test fails the device whatever the pass said, until reset
+        if (be->gpus[i]->memtest_fault.load(std::memory_order_relaxed)) {
+            out[i].flags |= B2DP_RES_MEMTEST;
+            out[i].healthy = 0;
+            be->gpus[i]->last_healthy = 0;
+        }
     return B2DP_OK;
 }
 
@@ -1190,6 +1199,7 @@ int cuda_probe_reset(CudaBackend* be, int device, std::string& err) {
         Gpu* g = be->gpus[i].get();
         if (g->broken) continue;
         g->xid_fault.store(0);  // operator acknowledgement: a latched Xid is cleared together with the buffers
+        g->memtest_fault.store(false);  // and so is a failed memory test
         cudaError_t ce = cudaSuccess;
         run_sync(g, [&] {
             probe_flush(g);
@@ -1312,6 +1322,247 @@ bool cuda_device_paths(CudaBackend* be, const std::string& id, std::vector<std::
         if (g->dev.id == id) { out.push_back("/dev/nvidia" + std::to_string(g->dev.card)); return true; }
     return false;
 }
+
+// ---- on-demand memory test (b2dp_memtest) ------------------------------------------------------
+// The march of hbm_memtest.cuh over the free HBM of one GPU, on that GPU's worker.  Every segment is freed before the
+// job ends, whatever happened.
+constexpr uint32_t kMemtestTimeoutMs = 60000;
+
+template <int MODE>
+static void launch_march(Gpu* g, const MarchSegs& segs, unsigned int tiles_per_seg, unsigned long long n_tiles,
+                         uint32_t inv, uint32_t delta, ProbeCtl* ctl, ProbeOut* out, unsigned long long seq) {
+    hbm_march_tma<kTmaCW, kTmaTileVec, kTmaStages, MODE>
+        <<<(int)g->sms * kTmaCtasPerSm, (kTmaCW + 1) * 32, kTmaSmem, g->stream>>>(segs, tiles_per_seg, n_tiles, inv,
+                                                                                  delta, ctl, out, seq);
+}
+
+template <int MODE>
+static cudaError_t march_attributes() {
+    cudaError_t e = cudaFuncSetAttribute(hbm_march_tma<kTmaCW, kTmaTileVec, kTmaStages, MODE>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTmaSmem);
+    if (e == cudaSuccess)
+        e = cudaFuncSetAttribute(hbm_march_tma<kTmaCW, kTmaTileVec, kTmaStages, MODE>,
+                                 cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    return e;
+}
+
+static void memtest_one(CudaBackend* be, Gpu* g, const b2dp_memtest_opts& o, uint32_t timeout_ms, b2dp_memtest_result* r,
+                        std::string* err) {
+    constexpr uint64_t kTileBytes = (uint64_t)kTmaTileVec * 16;
+    std::vector<uint64_t> got;       // sizes of the segments obtained
+    std::vector<void*> seg;
+    ProbeCtl* ctl = nullptr;
+    ProbeOut* out_h = nullptr;
+    ProbeOut* out_d = nullptr;
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    bool timed_out = false;
+    cudaError_t ce = cudaSuccess;
+    const char* where = "";
+    MemtestEvidence ev;
+    auto release = [&] {  // every path ends here: nothing the test allocated outlives it
+        if (g->stream) cudaStreamSynchronize(g->stream);
+        for (void* p : seg) cudaFree(p);
+        if (ctl) cudaFree(ctl);
+        if (out_h) cudaFreeHost(out_h);
+        if (e0) cudaEventDestroy(e0);
+        if (e1) cudaEventDestroy(e1);
+    };
+#define MT_TRY(x) if ((ce = (x)) != cudaSuccess) { where = #x; goto done; }
+    {
+        probe_flush(g);  // an armed heartbeat pass must not run underneath
+        size_t free_b = 0, total_b = 0;
+        MT_TRY(cudaMemGetInfo(&free_b, &total_b));
+        r->free_before = free_b;
+        r->total_memory = total_b;
+        // the small blocks first: they must not be what fails once the segments have taken the memory
+        MT_TRY(cudaMalloc(&ctl, kMarchElements * sizeof(ProbeCtl)));
+        MT_TRY(cudaHostAlloc(&out_h, kMarchElements * sizeof(ProbeOut), cudaHostAllocMapped));
+        memset(out_h, 0, kMarchElements * sizeof(ProbeOut));
+        MT_TRY(cudaHostGetDevicePointer(&out_d, out_h, 0));
+        {
+            ProbeCtl init[kMarchElements] = {};
+            for (auto& c : init) { c.first_bad = ~0ull; c.t_start_ns = ~0ull; }
+            MT_TRY(cudaMemcpy(ctl, init, sizeof init, cudaMemcpyHostToDevice));
+        }
+        MT_TRY(cudaEventCreate(&e0));
+        MT_TRY(cudaEventCreate(&e1));
+        MT_TRY(march_attributes<MARCH_WRITE>());
+        MT_TRY(march_attributes<MARCH_READ_WRITE>());
+        MT_TRY(march_attributes<MARCH_READ>());
+        const std::vector<uint64_t> plan = memtest_plan(free_b, total_b, o.reserve_bytes, o.max_bytes);
+        if (plan.empty()) r->flags |= B2DP_MT_EMPTY;
+        for (uint64_t bytes : plan) {  // a tenant may allocate meanwhile: test what was obtained
+            void* p = nullptr;
+            const cudaError_t a = cudaMalloc(&p, bytes);
+            if (a != cudaSuccess) {
+                cudaGetLastError();
+                r->flags |= B2DP_MT_PARTIAL;
+                break;
+            }
+            seg.push_back(p);
+            got.push_back(bytes);
+        }
+        r->n_segments = (int32_t)got.size();
+        for (uint64_t b : got) r->bytes_tested += b;
+        if (got.empty()) { ev.launch_ok = true; goto done; }  // nothing to test
+
+        MarchSegs segs{};
+        for (size_t k = 0; k < got.size(); ++k) {
+            segs.base[k] = static_cast<uint4*>(seg[k]);
+            segs.seed[k] = memtest_segment_seed(r->seed, (uint32_t)k);
+        }
+        const unsigned int tiles_per_seg = (unsigned int)(got[0] / kTileBytes);
+        const unsigned long long n_tiles = r->bytes_tested / kTileBytes;
+        const unsigned long long n_words = r->bytes_tested / 4, seg_words = got[0] / 4;
+        unsigned long long corr0 = 0, unc0 = 0;
+        const bool ecc = g->nvh && be->nvml.ecc_total && be->nvml.ecc_total(g->nvh, 1, 0, &unc0) == 0 &&
+                         be->nvml.ecc_total(g->nvh, 0, 0, &corr0) == 0;
+        if (!ecc) r->flags |= B2DP_MT_NO_ECC;
+
+        MT_TRY(cudaEventRecord(e0, g->stream));
+        launch_march<MARCH_WRITE>(g, segs, tiles_per_seg, n_tiles, 0u, 0u, ctl + 0, out_d + 0, 1);
+        if (o.fault_mask) {
+            if (o.fault_word < n_words) {
+                const unsigned long long s = o.fault_word / seg_words;
+                hbm_poke<<<1, 1, 0, g->stream>>>(static_cast<uint32_t*>(seg[s]), o.fault_word - s * seg_words, o.fault_mask);
+            } else {
+                r->err = B2DP_E_INVAL;  // not injected; the test runs as it would without the hook
+            }
+        }
+        launch_march<MARCH_READ_WRITE>(g, segs, tiles_per_seg, n_tiles, 0u, ~0u, ctl + 1, out_d + 1, 2);
+        launch_march<MARCH_READ_WRITE>(g, segs, tiles_per_seg, n_tiles, ~0u, ~0u, ctl + 2, out_d + 2, 3);
+        launch_march<MARCH_READ>(g, segs, tiles_per_seg, n_tiles, 0u, 0u, ctl + 3, out_d + 3, 4);
+        MT_TRY(cudaGetLastError());
+        MT_TRY(cudaEventRecord(e1, g->stream));
+        const auto deadline = std::chrono::steady_clock::now() + std::chrono::milliseconds(timeout_ms);
+        for (;;) {
+            const cudaError_t q = cudaEventQuery(e1);
+            if (q == cudaSuccess) break;
+            if (q != cudaErrorNotReady) { ce = q; where = "march"; goto done; }
+            if (std::chrono::steady_clock::now() > deadline) { timed_out = true; break; }
+            std::this_thread::sleep_for(std::chrono::microseconds(200));
+        }
+        // past the deadline the verdict is made, but the memory can only be returned once the kernels are done
+        MT_TRY(cudaEventSynchronize(e1));
+        MT_TRY(cudaEventElapsedTime(&r->ms, e0, e1));
+        if (ecc) {
+            unsigned long long corr1 = corr0, unc1 = unc0;
+            be->nvml.ecc_total(g->nvh, 1, 0, &unc1);
+            be->nvml.ecc_total(g->nvh, 0, 0, &corr1);
+            r->ecc_uncorrected = unc1 > unc0 ? unc1 - unc0 : 0;
+            r->ecc_corrected = corr1 > corr0 ? corr1 - corr0 : 0;
+        }
+        unsigned rc_corr = 0, rc_unc = 0, pending = 0, failed = 0;
+        if (g->nvh && be->nvml.remapped_rows && be->nvml.remapped_rows(g->nvh, &rc_corr, &rc_unc, &pending, &failed) == 0) {
+            ev.remap_failed = failed != 0;
+            ev.remap_pending = pending != 0;
+        }
+        ev.ecc_uncorrected = r->ecc_uncorrected;
+        if (r->ecc_corrected) r->flags |= B2DP_MT_ECC_CORRECTED;
+        if (r->ecc_uncorrected || ev.remap_failed || ev.remap_pending) r->flags |= B2DP_MT_ECC;
+        std::atomic_thread_fence(std::memory_order_acquire);
+        bool seq_ok = true;
+        r->first_bad_word = ~0ull;
+        for (int k = 0; k < kMarchElements; ++k) {
+            ProbeOut po;
+            memcpy(&po, (const void*)&out_h[k], sizeof po);  // published by the element's last CTA; the stream is done
+            seq_ok = seq_ok && po.seq == (unsigned long long)(k + 1);
+            ev.mismatches[k] = r->mismatches[k] = po.mismatches;
+            ev.checksum[k] = po.checksum;
+            if (po.mismatches && po.first_bad < r->first_bad_word) r->first_bad_word = po.first_bad;
+        }
+        ev.expected[1] = ev.expected[3] = memtest_expected_checksum(got, r->seed, 0u);
+        ev.expected[2] = memtest_expected_checksum(got, r->seed, ~0u);
+        ev.launch_ok = seq_ok && !timed_out;
+        if (r->ms > 0) r->gbs = (float)(6.0 * (double)r->bytes_tested / (double)r->ms * 1e-6);
+    }
+done:
+#undef MT_TRY
+    release();
+    if (ce != cudaSuccess) {
+        cudaGetLastError();
+        r->err = B2DP_E_CUDA;
+        r->healthy = 0;
+        *err = cuda_err(where, ce) + " on " + g->dev.id;
+    } else if (timed_out) {
+        r->err = B2DP_E_TIMEOUT;
+        r->healthy = 0;
+    } else {
+        r->healthy = memtest_healthy(ev) ? 1 : 0;
+    }
+}
+
+static bool cuda_memtest_latched(CudaBackend* be) {
+    for (auto& g : be->gpus)
+        if (g->memtest_fault.load()) return true;
+    return false;
+}
+
+static int cuda_memtest(CudaBackend* be, int device, const b2dp_memtest_opts* opts, std::vector<b2dp_memtest_result>& out,
+                        std::string& err) {
+    if (be->units) {
+        err = "the memory test runs in-process only (not with probe=helpers / probe=off / MIG)";
+        return B2DP_E_UNSUPPORTED;
+    }
+    if (device < -1 || device >= (int)be->gpus.size()) { err = "device index out of range"; return B2DP_E_INVAL; }
+    const b2dp_memtest_opts o = opts ? *opts : b2dp_memtest_opts{};
+    const uint32_t timeout_ms = o.timeout_ms ? o.timeout_ms : kMemtestTimeoutMs;
+    bool latched = false;
+    {
+        std::lock_guard<std::mutex> pl(be->probe_mu);  // a heartbeat waits for a running memory test
+        const uint32_t seed = (uint32_t)std::chrono::steady_clock::now().time_since_epoch().count() * kPatternMul;
+        std::vector<size_t> sel;
+        for (size_t i = 0; i < be->gpus.size(); ++i) if (device < 0 || (int)i == device) sel.push_back(i);
+        out.assign(sel.size(), b2dp_memtest_result{});
+        std::vector<std::string> errs(sel.size());
+        std::vector<std::shared_ptr<Completion>> cs(sel.size());
+        for (size_t k = 0; k < sel.size(); ++k) {
+            Gpu* g = be->gpus[sel[k]].get();
+            b2dp_memtest_result* r = &out[k];
+            r->device = (int32_t)sel[k];
+            r->seed = seed ^ ((uint32_t)sel[k] << 16);
+            r->first_bad_word = ~0ull;
+            r->total_memory = (uint64_t)g->vram;
+            if (g->broken) { r->err = B2DP_E_CUDA; errs[k] = g->broken_reason + " on " + g->dev.id; continue; }
+            if (!(o.flags & B2DP_MT_EVEN_IF_BUSY) && be->nvml.ok && be->nvml.running_procs && g->nvh) {
+                unsigned cnt = 0;
+                const int nrc = be->nvml.running_procs(g->nvh, &cnt, nullptr);  // count only (INSUFFICIENT_SIZE = 7)
+                if ((nrc == 0 || nrc == 7) && cnt > 1) {                       // this process holds one context itself
+                    r->flags |= B2DP_MT_SKIPPED_BUSY;
+                    r->healthy = g->last_healthy;
+                    continue;
+                }
+            }
+            std::string* e = &errs[k];
+            cs[k] = post(g, [be, g, o, timeout_ms, r, e] { memtest_one(be, g, o, timeout_ms, r, e); });
+        }
+        for (size_t k = 0; k < sel.size(); ++k) {
+            if (cs[k]) cs[k]->wait();  // no deadline here: the segments must be back before the call returns
+            if (!errs[k].empty()) err = errs[k];
+            if (!cs[k]) continue;       // skipped (busy) or never set up: nothing ran, nothing is latched
+            Gpu* g = be->gpus[sel[k]].get();
+            const b2dp_memtest_result& r = out[k];
+            if (!r.healthy) { g->memtest_fault.store(true); latched = true; }
+            logf(r.healthy ? 0 : 2, "%s memtest: %s, %llu MiB in %d segment(s)%s, mismatches %llu/%llu/%llu, first bad word %lld, "
+                 "ECC corrected %llu uncorrected %llu%s, %.1f ms, %.0f GB/s%s", g->dev.id.c_str(),
+                 r.healthy ? "Healthy" : "Unhealthy (latched)", (unsigned long long)(r.bytes_tested >> 20), r.n_segments,
+                 (r.flags & B2DP_MT_PARTIAL) ? " (partial)" : "", (unsigned long long)r.mismatches[1],
+                 (unsigned long long)r.mismatches[2], (unsigned long long)r.mismatches[3], (long long)r.first_bad_word,
+                 (unsigned long long)r.ecc_corrected, (unsigned long long)r.ecc_uncorrected,
+                 (r.flags & B2DP_MT_NO_ECC) ? " (not available)" : "", r.ms, r.gbs,
+                 r.err == B2DP_E_TIMEOUT ? ", timed out" : "");
+        }
+    }
+    // like the Xid latch: running ListAndWatch loops send a heartbeat now (no backend lock is held while they do)
+    if (latched) be->fire_health_event();
+    return B2DP_OK;
+}
+
+// registered when the library is loaded, before any entry point can run (internal.hpp MemtestHooks)
+[[maybe_unused]] static const bool kMemtestRegistered = [] {
+    memtest_hooks() = MemtestHooks{cuda_memtest, cuda_memtest_latched};
+    return true;
+}();
 
 // ---- P2P matrix ------------------------------------------------------------------------------
 constexpr float kNvlinkRefGbs = 450.f, kNvlinkClassFraction = 0.25f;  // oracle/probe.py

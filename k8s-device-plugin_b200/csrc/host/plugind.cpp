@@ -49,6 +49,9 @@ struct Flags {
     double start_retry_wait = 3.0;                   // dpm/manager.go:19
     int link_check = 0;
     std::string exporter_socket;                     // optional: serve metricssvc.MetricsService here (health.go:36)
+    int memtest_at_start = 0;                        // 1: test the free HBM of every idle GPU before the first registration;
+                                                     // 2: also GPUs another process is using
+    unsigned long long memtest_max_bytes = 0;        // cap per GPU for that test (0 = all free memory above the reserve)
     bool version = false;
     bool labels_mode = false, reconcile = false, patch = false;
     std::string labels;                              // csv of generator names, or "all"
@@ -84,6 +87,8 @@ bool parse_flags(int argc, char** argv, Flags& f, std::string& err) {
         else if (name == "start_retry_wait") f.start_retry_wait = atof(val.c_str());
         else if (name == "link_check") f.link_check = atoi(val.c_str());
         else if (name == "exporter_socket") f.exporter_socket = val;
+        else if (name == "memtest_at_start") f.memtest_at_start = atoi(val.c_str());
+        else if (name == "memtest_max_bytes") f.memtest_max_bytes = strtoull(val.c_str(), nullptr, 0);
         else if (name == "labels") { f.labels_mode = true; f.labels = val; }
         else { err = "flag provided but not defined: -" + name; return false; }
     }
@@ -476,6 +481,32 @@ int labels_main(const Flags& fl) {
     return 0;
 }
 
+// -memtest_at_start=1: test the free HBM of every GPU once, after open and before the first registration.  A failed
+// device stays latched Unhealthy; the watch loop reports it with a heartbeat right after the initial list.
+void run_memtest(b2dp_ctx* ctx, const Flags& fl) {
+    b2dp_memtest_opts o{};
+    o.max_bytes = fl.memtest_max_bytes;
+    if (fl.memtest_at_start >= 2) o.flags |= B2DP_MT_EVEN_IF_BUSY;
+    b2dp_memtest_result res[64];
+    int n = 0;
+    const int rc = b2dp_memtest(ctx, -1, &o, res, 64, &n);
+    if (rc != B2DP_OK) {
+        logf("memtest at start not run: %s (%s)", b2dp_strerror(rc), b2dp_last_error(ctx));
+        return;
+    }
+    std::vector<b2dp_device> devs(n > 0 ? n : 1);
+    int nd = 0;
+    if (b2dp_enumerate(ctx, devs.data(), (int)devs.size(), &nd) != B2DP_OK) nd = 0;
+    for (int i = 0; i < n; ++i) {
+        const b2dp_memtest_result& r = res[i];
+        logf("memtest %s: %s, %llu bytes in %d segment(s), flags 0x%x, mismatches %llu/%llu/%llu, ECC corrected %llu "
+             "uncorrected %llu, %.1f ms, %.0f GB/s", r.device < nd ? devs[r.device].id : "?",
+             r.healthy ? "Healthy" : "Unhealthy", (unsigned long long)r.bytes_tested, r.n_segments, r.flags,
+             (unsigned long long)r.mismatches[1], (unsigned long long)r.mismatches[2], (unsigned long long)r.mismatches[3],
+             (unsigned long long)r.ecc_corrected, (unsigned long long)r.ecc_uncorrected, r.ms, r.gbs);
+    }
+}
+
 }  // namespace
 
 int main(int argc, char** argv) {
@@ -506,6 +537,7 @@ int main(int argc, char** argv) {
     b2dp_ctx* ctx = nullptr;
     int rc = b2dp_open(fl.backend.c_str(), &ctx);
     if (rc != B2DP_OK) { logf("open %s: %s (%s)", fl.backend.c_str(), b2dp_strerror(rc), b2dp_last_error(nullptr)); return 1; }
+    if (fl.memtest_at_start) run_memtest(ctx, fl);
     char names[64][64];
     int n_res = 0;
     rc = b2dp_resource_list(ctx, fl.strategy.c_str(), names, 64, &n_res);  // main.go:141-146

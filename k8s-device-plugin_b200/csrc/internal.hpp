@@ -143,4 +143,16 @@ bool cuda_device_paths(CudaBackend*, const std::string& id, std::vector<std::str
 // xid=1: called (from a backend thread, or from b2dp_probe_inject_fault) when a device-level Xid has been latched
 void cuda_set_health_event_callback(CudaBackend*, std::function<void()> fn);
 
+// The on-demand memory test is an optional capability of the cuda backend: a build of the library whose backend has
+// none (the CPU-only build of ctx.cpp the sanitizer tests link against a stand-in backend) simply leaves these null,
+// and b2dp_memtest then returns B2DP_E_UNSUPPORTED.  cuda_backend.cu fills them in during static initialisation.
+struct MemtestHooks {
+    // b2dp_memtest on `device` (-1 = all); B2DP_E_UNSUPPORTED without the in-process probe
+    int (*run)(CudaBackend*, int device, const b2dp_memtest_opts* opts, std::vector<b2dp_memtest_result>& out,
+               std::string& err) = nullptr;
+    // true while any device carries a latched memtest failure (cleared by b2dp_probe_reset)
+    bool (*latched)(CudaBackend*) = nullptr;
+};
+MemtestHooks& memtest_hooks();  // ctx.cpp
+
 }  // namespace b2dp

@@ -7,7 +7,7 @@
 //       -Wl,-rpath,'$ORIGIN/../k8s-device-plugin_b200' -o tools/b200dp_cli
 //
 //   b200dp_cli <backend-uri> enumerate | health | cycle [steps [idle_ms]] | probe [steps] | resources <single|mixed>
-//                            | labels <csv> | alloc <size> | p2p
+//                            | labels <csv> | alloc <size> | p2p | memtest [max_bytes]
 #include <algorithm>
 #include <chrono>
 #include <ctime>
@@ -133,6 +133,25 @@ int main(int argc, char** argv) {
             for (int j = 0; j < n; ++j) printf("%7.1f/%-2d ", gbs[(size_t)i * n + j], lt[(size_t)i * n + j]);
             printf("\n");
         }
+    } else if (cmd == "memtest") {  // one line per device; exit status 1 if any device is Unhealthy
+        b2dp_memtest_opts mo{};
+        mo.max_bytes = argc > 3 ? strtoull(argv[3], nullptr, 0) : 0;
+        std::vector<b2dp_memtest_result> res(n ? n : 1);
+        int m = 0;
+        if ((rc = b2dp_memtest(ctx, -1, &mo, res.data(), (int)res.size(), &m)) != B2DP_OK) return die(ctx, "b2dp_memtest", rc);
+        int bad = 0;
+        for (int i = 0; i < m; ++i) {
+            const b2dp_memtest_result& r = res[i];
+            printf("%s %s err=%d flags=0x%x bytes=%llu segments=%d mismatches=%llu,%llu,%llu,%llu first_bad=%lld "
+                   "ecc_corrected=%llu ecc_uncorrected=%llu ms=%.2f gbs=%.0f\n",
+                   devs[r.device].id, r.healthy ? "Healthy" : "Unhealthy", r.err, r.flags, (unsigned long long)r.bytes_tested,
+                   r.n_segments, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
+                   (unsigned long long)r.mismatches[2], (unsigned long long)r.mismatches[3], (long long)r.first_bad_word,
+                   (unsigned long long)r.ecc_corrected, (unsigned long long)r.ecc_uncorrected, r.ms, r.gbs);
+            bad += !r.healthy;
+        }
+        b2dp_close(ctx);
+        return bad ? 1 : 0;
     } else {
         fprintf(stderr, "unknown command %s\n", cmd.c_str());
         b2dp_close(ctx);
