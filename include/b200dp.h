@@ -270,6 +270,8 @@ typedef struct b2dp_probe_result {
                                       last b2dp_probe_reset) => Unhealthy, sticky */
 #define B2DP_RES_MEMTEST 0x200u    /* a b2dp_memtest of this device failed or timed out since open (or the last
                                       b2dp_probe_reset) => Unhealthy, sticky */
+#define B2DP_RES_COMPUTE 0x400u    /* a b2dp_compute_test of this device failed or timed out since open (or the last
+                                      b2dp_probe_reset) => Unhealthy, sticky */
 
 /* Replaces the exporter round trip getGPUHealth (exporter/health.go:42-82) and the evidence behind simpleHealthCheck
  * (plugin.go:161-206): launch the probe on every GPU of the context concurrently (one worker thread + stream per
@@ -280,8 +282,8 @@ B2DP_API int b2dp_probe_health(b2dp_ctx *ctx, const b2dp_probe_opts *opts, b2dp_
  * NEXT probe of `device` will read.  word_index == UINT64_MAX instead queues a synthetic critical-Xid
  * event numbered `mask` for `device` (seen by contexts opened with xid=1).  The reference has no equivalent. */
 B2DP_API int b2dp_probe_inject_fault(b2dp_ctx *ctx, int device, uint64_t word_index, uint32_t mask);
-/* Re-fill the probe buffers of `device` (-1 = all) with a clean pattern; also clears a latched Xid and a latched memtest
- * failure. */
+/* Re-fill the probe buffers of `device` (-1 = all) with a clean pattern; also clears a latched Xid, a latched memtest
+ * failure and a latched compute-test failure. */
 B2DP_API int b2dp_probe_reset(b2dp_ctx *ctx, int device);
 /* Set the bandwidth ceiling (gbs_ref) of `device` (-1 = all) the fractional floor refers to, e.g. to the site's measured
  * HBM peak; gbs_ref <= 0 restores the device's own calibration.  Also how tests move a device across the 0.8 line. */
@@ -357,6 +359,54 @@ typedef struct b2dp_memtest_result {
  * B2DP_MT_EVEN_IF_BUSY.  cuda: backend with the in-process probe only; B2DP_E_UNSUPPORTED otherwise. */
 B2DP_API int b2dp_memtest(b2dp_ctx *ctx, int device, const b2dp_memtest_opts *opts, b2dp_memtest_result *out, int cap,
                           int *n);
+
+/* ---- on-demand tensor-core self-test (feeds the same per-GPU verdict as the probe) ---- */
+typedef struct b2dp_compute_test_opts {
+    uint32_t duration_ms;    /* per format; 0 = 1000 (every CTA still completes at least one round) */
+    uint32_t timeout_ms;     /* per-call deadline; 0 = 10000 + 6 * duration */
+    uint32_t flags;          /* B2DP_CT_EVEN_IF_BUSY */
+    int32_t fault_sm;        /* test hook: CTAs on the SM with this %smid flip fault_mask in one accumulator element of
+                                their first comparison, in every format; ignored when fault_mask = 0 */
+    uint32_t fault_mask;
+    uint32_t reserved;
+} b2dp_compute_test_opts;
+#define B2DP_CT_EVEN_IF_BUSY 0x1u  /* test a GPU even while another process uses it (default: skip it) */
+
+#define B2DP_CT_BF16 0             /* format index of mismatches[] / ms[] / tflops[] / first_bad_format */
+#define B2DP_CT_FP8 1
+#define B2DP_CT_INT8 2
+typedef struct b2dp_compute_test_result {
+    int32_t device;             /* index into b2dp_enumerate() order */
+    int32_t healthy;            /* 1 Healthy, 0 Unhealthy (a failure is latched: B2DP_RES_COMPUTE) */
+    int32_t err;                /* B2DP_OK | B2DP_E_CUDA | B2DP_E_TIMEOUT */
+    uint32_t flags;             /* B2DP_CT_* */
+    uint32_t seed;              /* operand seed of the test */
+    int32_t sm_count;           /* the device's SM count */
+    int32_t nsmid;              /* %nsmid: SM ids lie in [0, nsmid) */
+    int32_t sms_covered;        /* distinct SM ids on which every format ran at least one CTA */
+    uint64_t bad_sm_mask[4];    /* bit s: a CTA on the SM with %smid s had a mismatch (any format) */
+    uint64_t mismatches[3];     /* per format: comparisons (one result tile of one CTA) that differed from the host's */
+    int32_t first_bad_sm;       /* lowest bad SM id of the first format with a mismatch; -1 if none */
+    int32_t first_bad_format;   /* B2DP_CT_BF16 / _FP8 / _INT8; -1 if none */
+    int32_t first_bad_tile;     /* first mismatching operand tile of that SM's first bad CTA; -1 if none */
+    float ms[3];                /* per format: CUDA-event time of the launch */
+    float tflops[3];            /* per format: 2 * M * N * K * result tiles compared / ms (TOPS for INT8) */
+} b2dp_compute_test_result;
+#define B2DP_CT_SKIPPED_BUSY 0x1u      /* another process uses the GPU: nothing ran, nothing latched;
+                                          healthy = the last heartbeat verdict */
+#define B2DP_CT_PARTIAL_COVERAGE 0x2u  /* sms_covered < sm_count: some SM ran no CTA of some format (reported, not failed) */
+
+/* An on-demand check of the SMs' tensor cores on `device` (-1 = every GPU, concurrently on their workers): evidence
+ * behind the per-GPU verdict the exporter round trip supplies in the reference (exporter/health.go:42-82), merged the
+ * same way (exporter/health.go:86-106) through the sticky B2DP_RES_COMPUTE bit.  Per GPU and per format (BF16, FP8
+ * e4m3, INT8) one launch of tc_selftest.cuh fills every SM with warpgroup GEMMs (wgmma) on host-generated integer
+ * operands for duration_ms, compares every result tile with the exact product the host computed, and reports which SM
+ * ids and formats disagreed.  Healthy iff every launch succeeded before the deadline and every CTA reported complete
+ * rounds with no mismatch.  Every allocation is released before the call returns, on every path.  The probe lock is
+ * held throughout: a heartbeat waits for a running test.  A GPU another process uses is skipped (B2DP_CT_SKIPPED_BUSY)
+ * unless B2DP_CT_EVEN_IF_BUSY.  cuda: backend with the in-process probe only; B2DP_E_UNSUPPORTED otherwise. */
+B2DP_API int b2dp_compute_test(b2dp_ctx *ctx, int device, const b2dp_compute_test_opts *opts,
+                               b2dp_compute_test_result *out, int cap, int *n);
 
 /* exporter/health.go:86-106 PopulatePerGPUDHealth(devs, defaultHealth) merge rule.
  * have_source = 0 reproduces "exporter socket absent / RPC failed" (every device gets the

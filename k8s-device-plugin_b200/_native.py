@@ -41,6 +41,10 @@ LW_INITIAL, LW_HEARTBEAT, LW_EXTERNAL_SOURCE, LW_NO_PROBE, LW_LINK_CHECK = 1, 2,
 RES_MEMTEST = 0x200
 MT_EVEN_IF_BUSY = 1
 MT_SKIPPED_BUSY, MT_PARTIAL, MT_ECC_CORRECTED, MT_ECC, MT_NO_ECC, MT_EMPTY = 1, 2, 4, 8, 0x10, 0x20
+RES_COMPUTE = 0x400
+CT_EVEN_IF_BUSY = 1
+CT_SKIPPED_BUSY, CT_PARTIAL_COVERAGE = 1, 2
+CT_BF16, CT_FP8, CT_INT8 = 0, 1, 2
 
 Id64 = C.c_char * 64
 
@@ -122,6 +126,19 @@ class MemtestResult(C.Structure):
                 ("ecc_corrected", C.c_uint64), ("ecc_uncorrected", C.c_uint64), ("ms", C.c_float), ("gbs", C.c_float)]
 
 
+class ComputeTestOpts(C.Structure):
+    _fields_ = [("duration_ms", C.c_uint32), ("timeout_ms", C.c_uint32), ("flags", C.c_uint32), ("fault_sm", C.c_int32),
+                ("fault_mask", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+class ComputeTestResult(C.Structure):
+    _fields_ = [("device", C.c_int32), ("healthy", C.c_int32), ("err", C.c_int32), ("flags", C.c_uint32),
+                ("seed", C.c_uint32), ("sm_count", C.c_int32), ("nsmid", C.c_int32), ("sms_covered", C.c_int32),
+                ("bad_sm_mask", C.c_uint64 * 4), ("mismatches", C.c_uint64 * 3), ("first_bad_sm", C.c_int32),
+                ("first_bad_format", C.c_int32), ("first_bad_tile", C.c_int32), ("ms", C.c_float * 3),
+                ("tflops", C.c_float * 3)]
+
+
 if not os.path.exists(LIB_PATH):
     raise ImportError(
         "libb200dp.so is not built: run `python -c 'import __graft_entry__ as g; g.build()'` "
@@ -161,6 +178,7 @@ SIGNATURES = {
     "b2dp_probe_reset": (_i, [_vp, _i]),
     "b2dp_probe_peek": (_i, [_vp, _i, C.c_uint64, _P(C.c_uint32), C.c_uint64]),
     "b2dp_memtest": (_i, [_vp, _i, _P(MemtestOpts), _P(MemtestResult), _i, _ip]),
+    "b2dp_compute_test": (_i, [_vp, _i, _P(ComputeTestOpts), _P(ComputeTestResult), _i, _ip]),
     "b2dp_probe_set_ref": (_i, [_vp, _i, C.c_float]),
     "b2dp_probe_describe": (_i, [_vp, _i, _P(ProbeInfo)]),
     "b2dp_expected_checksum": (_i, [C.c_uint64, C.c_uint32, _P(C.c_uint64)]),

@@ -47,6 +47,28 @@ class MemtestResult:
 
 
 @dataclass
+class ComputeTestResult:
+    device: int
+    healthy: bool
+    err: int
+    flags: int
+    seed: int
+    sm_count: int
+    nsmid: int
+    sms_covered: int               # SM ids on which every format ran at least one CTA
+    bad_sm_mask: List[int]         # 4 x 64 bits over %smid
+    mismatches: List[int]          # per format: BF16, FP8, INT8
+    first_bad_sm: int
+    first_bad_format: int
+    first_bad_tile: int
+    ms: List[float]
+    tflops: List[float]            # 2 M N K x result tiles compared / ms (TOPS for INT8)
+
+    def bad_sms(self) -> List[int]:
+        return [s for s in range(256) if (self.bad_sm_mask[s // 64] >> (s % 64)) & 1]
+
+
+@dataclass
 class CycleStats:
     n_devices: int
     n_unhealthy: int
@@ -189,6 +211,20 @@ class Context:
         return [MemtestResult(r.device, bool(r.healthy), r.err, r.flags, r.seed, r.n_segments, r.bytes_tested,
                               r.free_before, r.total_memory, list(r.mismatches), r.first_bad_word, r.ecc_corrected,
                               r.ecc_uncorrected, r.ms, r.gbs) for r in arr[:n]]
+
+    def compute_test(self, device: int = -1, duration_ms: int = 0, timeout_ms: int = 0, even_if_busy: bool = False,
+                     fault_sm: int = -1, fault_mask: int = 0) -> List[ComputeTestResult]:
+        """On-demand tensor-core self-test of `device` (-1 = every GPU, b2dp_compute_test): BF16, FP8 and INT8 warpgroup
+        GEMMs on every SM for duration_ms each (0 = 1000), every result compared bit for bit with the host's exact
+        product.  A failure is latched: later probe results carry RES_COMPUTE and are Unhealthy until probe_reset().
+        fault_sm / fault_mask is a test hook that flips bits of one accumulator on the SM with that %smid."""
+        opts = N.ComputeTestOpts(duration_ms, timeout_ms, N.CT_EVEN_IF_BUSY if even_if_busy else 0, fault_sm, fault_mask, 0)
+        rc, arr, n = N.grow_call(lambda cap: (N.ComputeTestResult * cap)(),
+                                 lambda a, cap, pn: N.lib.b2dp_compute_test(self._h, device, C.byref(opts), a, cap, pn))
+        N.check(rc, self._h)
+        return [ComputeTestResult(r.device, bool(r.healthy), r.err, r.flags, r.seed, r.sm_count, r.nsmid, r.sms_covered,
+                                  list(r.bad_sm_mask), list(r.mismatches), r.first_bad_sm, r.first_bad_format,
+                                  r.first_bad_tile, list(r.ms), list(r.tflops)) for r in arr[:n]]
 
     # ---- ListAndWatch --------------------------------------------------------------------
     def list_and_watch(self, resource: str = "gpu", flags: int = N.LW_INITIAL, external: Optional[Dict[str, bool]] = None,

@@ -53,8 +53,8 @@ struct b2dp_ctx {
 static int fail(int code, const std::string& msg) { t_last_error = msg; return code; }
 
 namespace b2dp {
-MemtestHooks& memtest_hooks() {
-    static MemtestHooks hooks;
+DiagHooks& diag_hooks() {
+    static DiagHooks hooks;
     return hooks;
 }
 }  // namespace b2dp
@@ -452,12 +452,34 @@ extern "C" int b2dp_memtest(b2dp_ctx* c, int device, const b2dp_memtest_opts* op
     if (*n && !out) return B2DP_E_INVAL;
     std::vector<b2dp_memtest_result> res;
     std::string err;
-    const MemtestHooks& mt = memtest_hooks();
-    if (!mt.run) return fail(B2DP_E_UNSUPPORTED, "this build of the library has no memory test");
-    int rc = mt.run(c->cuda, device, opts, res, err);
+    const DiagHooks& dh = diag_hooks();
+    if (!dh.memtest) return fail(B2DP_E_UNSUPPORTED, "this build of the library has no memory test");
+    int rc = dh.memtest(c->cuda, device, opts, res, err);
     if (rc != B2DP_OK) return fail(rc, err);
     *n = (int)res.size();
     memcpy(out, res.data(), res.size() * sizeof(b2dp_memtest_result));
+    return B2DP_OK;
+}
+
+extern "C" int b2dp_compute_test(b2dp_ctx* c, int device, const b2dp_compute_test_opts* opts,
+                                 b2dp_compute_test_result* out, int cap, int* n) {
+    if (!c || !n || cap < 0) return B2DP_E_INVAL;
+    if (c->kind != b2dp_ctx::CUDA)
+        return fail(B2DP_E_UNSUPPORTED, "the compute self-test needs the cuda: backend (there is no CPU fallback)");
+    // the capacity is checked before the test runs: its results cannot be produced a second time for free
+    const int count = cuda_device_count(c->cuda);
+    if (device < -1 || device >= count) return fail(B2DP_E_INVAL, "device index out of range");
+    *n = device < 0 ? count : 1;
+    if (*n > cap) return B2DP_E_NOSPC;
+    if (*n && !out) return B2DP_E_INVAL;
+    std::vector<b2dp_compute_test_result> res;
+    std::string err;
+    const DiagHooks& dh = diag_hooks();
+    if (!dh.compute_test) return fail(B2DP_E_UNSUPPORTED, "this build of the library has no compute self-test");
+    int rc = dh.compute_test(c->cuda, device, opts, res, err);
+    if (rc != B2DP_OK) return fail(rc, err);
+    *n = (int)res.size();
+    memcpy(out, res.data(), res.size() * sizeof(b2dp_compute_test_result));
     return B2DP_OK;
 }
 
@@ -644,10 +666,11 @@ static void watch_send(b2dp_watch* w, uint32_t flags) {
 
 static void watch_loop(b2dp_watch* w) {
     watch_send(w, B2DP_LW_INITIAL);
-    // The initial list says every device is Healthy (plugin.go:231-299).  A device whose memory test has failed is
-    // reported by one heartbeat right away, so the kubelet learns of it even without a ticker (-pulse=0).
-    const MemtestHooks& mt = memtest_hooks();
-    if (w->ctx->kind == b2dp_ctx::CUDA && mt.latched && mt.latched(w->ctx->cuda)) watch_send(w, B2DP_LW_HEARTBEAT);
+    // The initial list says every device is Healthy (plugin.go:231-299).  A device whose memory test or compute
+    // self-test has failed is reported by one heartbeat right away, so the kubelet learns of it even without a ticker
+    // (-pulse=0).
+    const DiagHooks& dh = diag_hooks();
+    if (w->ctx->kind == b2dp_ctx::CUDA && dh.latched && dh.latched(w->ctx->cuda)) watch_send(w, B2DP_LW_HEARTBEAT);
     auto next = std::chrono::steady_clock::now() + std::chrono::milliseconds(w->pulse_ms);
     for (;;) {
         {

@@ -35,6 +35,7 @@
 #include "memtest_math.hpp"
 #include "nvml_dyn.hpp"
 #include "pattern_math.hpp"
+#include "tc_selftest.cuh"
 #include "units_backend.hpp"
 
 namespace b2dp {
@@ -101,6 +102,7 @@ struct Gpu {
     bool xid_registered = false;
     std::atomic<unsigned long long> xid_fault{0};  // first critical Xid seen on this device (sticky, like a real fault)
     std::atomic<bool> memtest_fault{false};        // a b2dp_memtest failed or timed out (sticky until b2dp_probe_reset)
+    std::atomic<bool> compute_fault{false};        // a b2dp_compute_test failed or timed out (likewise)
     int last_healthy = 1;
     // worker
     std::thread th;
@@ -1110,6 +1112,12 @@ int cuda_probe(CudaBackend* be, const b2dp_probe_opts* opts, std::vector<b2dp_pr
             out[i].healthy = 0;
             be->gpus[i]->last_healthy = 0;
         }
+    for (size_t i = 0; i < n; ++i)  // and so does a failed compute self-test
+        if (be->gpus[i]->compute_fault.load(std::memory_order_relaxed)) {
+            out[i].flags |= B2DP_RES_COMPUTE;
+            out[i].healthy = 0;
+            be->gpus[i]->last_healthy = 0;
+        }
     return B2DP_OK;
 }
 
@@ -1200,6 +1208,7 @@ int cuda_probe_reset(CudaBackend* be, int device, std::string& err) {
         if (g->broken) continue;
         g->xid_fault.store(0);  // operator acknowledgement: a latched Xid is cleared together with the buffers
         g->memtest_fault.store(false);  // and so is a failed memory test
+        g->compute_fault.store(false);  // and a failed compute self-test
         cudaError_t ce = cudaSuccess;
         run_sync(g, [&] {
             probe_flush(g);
@@ -1492,10 +1501,13 @@ done:
     }
 }
 
-static bool cuda_memtest_latched(CudaBackend* be) {
-    for (auto& g : be->gpus)
-        if (g->memtest_fault.load()) return true;
-    return false;
+// NVML lists a compute process on the GPU other than this one (which holds a context itself).  Without NVML process
+// accounting the GPU counts as idle.
+static bool used_by_another_process(CudaBackend* be, Gpu* g) {
+    if (!be->nvml.ok || !be->nvml.running_procs || !g->nvh) return false;
+    unsigned cnt = 0;
+    const int nrc = be->nvml.running_procs(g->nvh, &cnt, nullptr);  // count only (INSUFFICIENT_SIZE = 7)
+    return (nrc == 0 || nrc == 7) && cnt > 1;
 }
 
 static int cuda_memtest(CudaBackend* be, int device, const b2dp_memtest_opts* opts, std::vector<b2dp_memtest_result>& out,
@@ -1524,14 +1536,10 @@ static int cuda_memtest(CudaBackend* be, int device, const b2dp_memtest_opts* op
             r->first_bad_word = ~0ull;
             r->total_memory = (uint64_t)g->vram;
             if (g->broken) { r->err = B2DP_E_CUDA; errs[k] = g->broken_reason + " on " + g->dev.id; continue; }
-            if (!(o.flags & B2DP_MT_EVEN_IF_BUSY) && be->nvml.ok && be->nvml.running_procs && g->nvh) {
-                unsigned cnt = 0;
-                const int nrc = be->nvml.running_procs(g->nvh, &cnt, nullptr);  // count only (INSUFFICIENT_SIZE = 7)
-                if ((nrc == 0 || nrc == 7) && cnt > 1) {                       // this process holds one context itself
-                    r->flags |= B2DP_MT_SKIPPED_BUSY;
-                    r->healthy = g->last_healthy;
-                    continue;
-                }
+            if (!(o.flags & B2DP_MT_EVEN_IF_BUSY) && used_by_another_process(be, g)) {
+                r->flags |= B2DP_MT_SKIPPED_BUSY;
+                r->healthy = g->last_healthy;
+                continue;
             }
             std::string* e = &errs[k];
             cs[k] = post(g, [be, g, o, timeout_ms, r, e] { memtest_one(be, g, o, timeout_ms, r, e); });
@@ -1558,9 +1566,201 @@ static int cuda_memtest(CudaBackend* be, int device, const b2dp_memtest_opts* op
     return B2DP_OK;
 }
 
-// registered when the library is loaded, before any entry point can run (internal.hpp MemtestHooks)
-[[maybe_unused]] static const bool kMemtestRegistered = [] {
-    memtest_hooks() = MemtestHooks{cuda_memtest, cuda_memtest_latched};
+// ---- on-demand tensor-core self-test (b2dp_compute_test) -------------------------------------------------------
+// One launch of tc_selftest.cuh per format on one GPU, on that GPU's worker.  The host builds every operand image and
+// every comparison value itself (compute_test_math.hpp): a health test must not ask the device under test for its own
+// reference values.  Every allocation is released before the job ends, whatever happened.
+constexpr uint32_t kComputeTestDefaultMs = 1000;
+
+using CtKernel = void (*)(const uint8_t*, const uint32_t*, unsigned long long, int, uint32_t, CtRecord*,
+                          unsigned long long, uint32_t*);
+static const CtKernel kCtKernels[kCtFormats] = {tc_selftest<CT_BF16, false>, tc_selftest<CT_FP8, false>,
+                                                tc_selftest<CT_INT8, false>};
+static const uint32_t kCtSmem[kCtFormats] = {CtShape<CT_BF16>::SMEM, CtShape<CT_FP8>::SMEM, CtShape<CT_INT8>::SMEM};
+
+static void compute_test_one(Gpu* g, const b2dp_compute_test_opts& o, uint32_t duration_ms, uint32_t timeout_ms,
+                             b2dp_compute_test_result* r, std::string* err) {
+    uint8_t* img[kCtFormats] = {};
+    uint32_t* chk[kCtFormats] = {};
+    CtRecord* rec_h = nullptr;
+    CtRecord* rec_d = nullptr;
+    cudaEvent_t ev[kCtFormats + 1] = {};
+    bool timed_out = false;
+    cudaError_t ce = cudaSuccess;
+    const char* where = "";
+    auto release = [&] {  // every path ends here: nothing the test allocated outlives it
+        if (g->stream) cudaStreamSynchronize(g->stream);
+        for (int f = 0; f < kCtFormats; ++f) {
+            if (img[f]) cudaFree(img[f]);
+            if (chk[f]) cudaFree(chk[f]);
+        }
+        if (rec_h) cudaFreeHost(rec_h);
+        for (cudaEvent_t e : ev)
+            if (e) cudaEventDestroy(e);
+    };
+#define CT_TRY(x) if ((ce = (x)) != cudaSuccess) { where = #x; goto done; }
+    {
+        probe_flush(g);  // an armed heartbeat pass must not run underneath
+        int grid[kCtFormats], off[kCtFormats + 1] = {0};
+        for (int f = 0; f < kCtFormats; ++f) {
+            CT_TRY(cudaFuncSetAttribute(kCtKernels[f], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kCtSmem[f]));
+            CT_TRY(cudaFuncSetAttribute(kCtKernels[f], cudaFuncAttributePreferredSharedMemoryCarveout, 100));
+            int per_sm = 0;
+            CT_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kCtKernels[f], kCtThreads, kCtSmem[f]));
+            grid[f] = (int)g->sms * (per_sm > 0 ? per_sm : 1);  // every CTA resident at once
+            off[f + 1] = off[f] + grid[f];
+        }
+        CT_TRY(cudaHostAlloc(&rec_h, (size_t)off[kCtFormats] * sizeof(CtRecord), cudaHostAllocMapped));
+        memset(rec_h, 0, (size_t)off[kCtFormats] * sizeof(CtRecord));
+        CT_TRY(cudaHostGetDevicePointer(&rec_d, rec_h, 0));
+        for (int f = 0; f < kCtFormats; ++f) {
+            std::vector<uint8_t> images((size_t)kCtTiles * kCtSmem[f]);
+            std::vector<uint32_t> checks((size_t)kCtTiles * kCtThreads);
+            CtTile t;
+            for (int tile = 0; tile < kCtTiles; ++tile) {
+                ct_build_tile(r->seed, f, tile, t);
+                memcpy(images.data() + (size_t)tile * kCtSmem[f], t.image.data(), kCtSmem[f]);
+                memcpy(checks.data() + (size_t)tile * kCtThreads, t.check, sizeof t.check);
+            }
+            CT_TRY(cudaMalloc(&img[f], images.size()));
+            CT_TRY(cudaMalloc(&chk[f], checks.size() * sizeof(uint32_t)));
+            CT_TRY(cudaMemcpy(img[f], images.data(), images.size(), cudaMemcpyHostToDevice));
+            CT_TRY(cudaMemcpy(chk[f], checks.data(), checks.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+        }
+        for (cudaEvent_t& e : ev) CT_TRY(cudaEventCreate(&e));
+
+        CT_TRY(cudaEventRecord(ev[0], g->stream));
+        for (int f = 0; f < kCtFormats; ++f) {
+            kCtKernels[f]<<<grid[f], kCtThreads, kCtSmem[f], g->stream>>>(
+                img[f], chk[f], (unsigned long long)duration_ms * 1000000ull, o.fault_sm, o.fault_mask, rec_d + off[f],
+                (unsigned long long)(f + 1), nullptr);
+            CT_TRY(cudaGetLastError());
+            CT_TRY(cudaEventRecord(ev[f + 1], g->stream));
+        }
+        const auto deadline = std::chrono::steady_clock::now() + std::chrono::milliseconds(timeout_ms);
+        for (;;) {
+            const cudaError_t q = cudaEventQuery(ev[kCtFormats]);
+            if (q == cudaSuccess) break;
+            if (q != cudaErrorNotReady) { ce = q; where = "tc_selftest"; goto done; }
+            if (std::chrono::steady_clock::now() > deadline) { timed_out = true; break; }
+            std::this_thread::sleep_for(std::chrono::milliseconds(1));
+        }
+        // past the deadline the verdict is made, but the buffers can only be released once the kernels are done
+        CT_TRY(cudaEventSynchronize(ev[kCtFormats]));
+        std::atomic_thread_fence(std::memory_order_acquire);
+
+        std::vector<CtRecord> recs[kCtFormats];
+        unsigned long long seq[kCtFormats];
+        std::vector<uint8_t> seen[kCtFormats];
+        for (int f = 0; f < kCtFormats; ++f) {
+            CT_TRY(cudaEventElapsedTime(&r->ms[f], ev[f], ev[f + 1]));
+            seq[f] = (unsigned long long)(f + 1);
+            recs[f].resize(grid[f]);
+            memcpy(recs[f].data(), (const void*)(rec_h + off[f]), (size_t)grid[f] * sizeof(CtRecord));
+            seen[f].assign(kCtMaxSmId, 0);
+            unsigned long long compared = 0;
+            int bad_sm = -1, bad_tile = -1;
+            for (const CtRecord& c : recs[f]) {
+                if (c.seq != seq[f]) continue;  // never arrived: fails the verdict below
+                r->nsmid = std::max<int32_t>(r->nsmid, (int32_t)c.nsmid);
+                compared += c.comparisons;
+                r->mismatches[f] += c.mismatches;
+                if (c.smid >= (uint32_t)kCtMaxSmId) continue;
+                seen[f][c.smid] = 1;
+                if (c.mismatches) {
+                    r->bad_sm_mask[c.smid / 64] |= 1ull << (c.smid % 64);
+                    if (bad_sm < 0 || (int)c.smid < bad_sm) { bad_sm = (int)c.smid; bad_tile = c.first_bad_tile; }
+                }
+            }
+            if (bad_sm >= 0 && r->first_bad_format < 0) {
+                r->first_bad_format = f;
+                r->first_bad_sm = bad_sm;
+                r->first_bad_tile = bad_tile;
+            }
+            if (r->ms[f] > 0) r->tflops[f] = (float)(2.0 * ct_macs_per_tile(f) * (double)compared / r->ms[f] * 1e-9);
+        }
+        for (int s = 0; s < kCtMaxSmId; ++s) r->sms_covered += seen[0][s] && seen[1][s] && seen[2][s];
+        if (r->sms_covered < r->sm_count) r->flags |= B2DP_CT_PARTIAL_COVERAGE;
+        r->healthy = compute_test_healthy(!timed_out, recs, seq) ? 1 : 0;
+    }
+done:
+#undef CT_TRY
+    release();
+    if (ce != cudaSuccess) {
+        cudaGetLastError();
+        r->err = B2DP_E_CUDA;
+        r->healthy = 0;
+        *err = cuda_err(where, ce) + " on " + g->dev.id;
+    } else if (timed_out) {
+        r->err = B2DP_E_TIMEOUT;
+        r->healthy = 0;
+    }
+}
+
+static int cuda_compute_test(CudaBackend* be, int device, const b2dp_compute_test_opts* opts,
+                             std::vector<b2dp_compute_test_result>& out, std::string& err) {
+    if (be->units) {
+        err = "the compute self-test runs in-process only (not with probe=helpers / probe=off / MIG)";
+        return B2DP_E_UNSUPPORTED;
+    }
+    if (device < -1 || device >= (int)be->gpus.size()) { err = "device index out of range"; return B2DP_E_INVAL; }
+    const b2dp_compute_test_opts o = opts ? *opts : b2dp_compute_test_opts{};
+    const uint32_t duration_ms = o.duration_ms ? o.duration_ms : kComputeTestDefaultMs;
+    const uint32_t timeout_ms = o.timeout_ms ? o.timeout_ms : 10000u + 6u * duration_ms;
+    bool latched = false;
+    {
+        std::lock_guard<std::mutex> pl(be->probe_mu);  // a heartbeat waits for a running self-test
+        const uint32_t seed = (uint32_t)std::chrono::steady_clock::now().time_since_epoch().count() * kPatternMul;
+        std::vector<size_t> sel;
+        for (size_t i = 0; i < be->gpus.size(); ++i) if (device < 0 || (int)i == device) sel.push_back(i);
+        out.assign(sel.size(), b2dp_compute_test_result{});
+        std::vector<std::string> errs(sel.size());
+        std::vector<std::shared_ptr<Completion>> cs(sel.size());
+        for (size_t k = 0; k < sel.size(); ++k) {
+            Gpu* g = be->gpus[sel[k]].get();
+            b2dp_compute_test_result* r = &out[k];
+            r->device = (int32_t)sel[k];
+            r->seed = seed ^ ((uint32_t)sel[k] << 16);
+            r->sm_count = (int32_t)g->sms;
+            r->first_bad_sm = r->first_bad_format = r->first_bad_tile = -1;
+            if (g->broken) { r->err = B2DP_E_CUDA; errs[k] = g->broken_reason + " on " + g->dev.id; continue; }
+            if (!(o.flags & B2DP_CT_EVEN_IF_BUSY) && used_by_another_process(be, g)) {
+                r->flags |= B2DP_CT_SKIPPED_BUSY;
+                r->healthy = g->last_healthy;
+                continue;
+            }
+            std::string* e = &errs[k];
+            cs[k] = post(g, [g, o, duration_ms, timeout_ms, r, e] { compute_test_one(g, o, duration_ms, timeout_ms, r, e); });
+        }
+        for (size_t k = 0; k < sel.size(); ++k) {
+            if (cs[k]) cs[k]->wait();  // no deadline here: the buffers must be released before the call returns
+            if (!errs[k].empty()) err = errs[k];
+            if (!cs[k]) continue;       // skipped (busy) or never set up: nothing ran, nothing is latched
+            Gpu* g = be->gpus[sel[k]].get();
+            const b2dp_compute_test_result& r = out[k];
+            if (!r.healthy) { g->compute_fault.store(true); latched = true; }
+            logf(r.healthy ? 0 : 2, "%s compute test: %s, SMs %d/%d, mismatches bf16/fp8/int8 %llu/%llu/%llu, first bad SM %d "
+                 "format %d tile %d, %.1f/%.1f/%.1f ms, %.0f/%.0f/%.0f TFLOP/s%s", g->dev.id.c_str(),
+                 r.healthy ? "Healthy" : "Unhealthy (latched)", r.sms_covered, r.sm_count,
+                 (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
+                 (unsigned long long)r.mismatches[2], r.first_bad_sm, r.first_bad_format, r.first_bad_tile, r.ms[0],
+                 r.ms[1], r.ms[2], r.tflops[0], r.tflops[1], r.tflops[2], r.err == B2DP_E_TIMEOUT ? ", timed out" : "");
+        }
+    }
+    // like the Xid latch: running ListAndWatch loops send a heartbeat now (no backend lock is held while they do)
+    if (latched) be->fire_health_event();
+    return B2DP_OK;
+}
+
+static bool cuda_diag_latched(CudaBackend* be) {
+    for (auto& g : be->gpus)
+        if (g->memtest_fault.load() || g->compute_fault.load()) return true;
+    return false;
+}
+
+// registered when the library is loaded, before any entry point can run (internal.hpp DiagHooks)
+[[maybe_unused]] static const bool kDiagRegistered = [] {
+    diag_hooks() = DiagHooks{cuda_memtest, cuda_compute_test, cuda_diag_latched};
     return true;
 }();
 

@@ -52,6 +52,8 @@ struct Flags {
     int memtest_at_start = 0;                        // 1: test the free HBM of every idle GPU before the first registration;
                                                      // 2: also GPUs another process is using
     unsigned long long memtest_max_bytes = 0;        // cap per GPU for that test (0 = all free memory above the reserve)
+    int compute_test_at_start = 0;                   // likewise for the tensor-core self-test (after the memtest if both)
+    unsigned compute_test_ms = 0;                    // its duration per format (0 = 1000 ms)
     bool version = false;
     bool labels_mode = false, reconcile = false, patch = false;
     std::string labels;                              // csv of generator names, or "all"
@@ -89,6 +91,8 @@ bool parse_flags(int argc, char** argv, Flags& f, std::string& err) {
         else if (name == "exporter_socket") f.exporter_socket = val;
         else if (name == "memtest_at_start") f.memtest_at_start = atoi(val.c_str());
         else if (name == "memtest_max_bytes") f.memtest_max_bytes = strtoull(val.c_str(), nullptr, 0);
+        else if (name == "compute_test_at_start") f.compute_test_at_start = atoi(val.c_str());
+        else if (name == "compute_test_ms") f.compute_test_ms = (unsigned)strtoul(val.c_str(), nullptr, 0);
         else if (name == "labels") { f.labels_mode = true; f.labels = val; }
         else { err = "flag provided but not defined: -" + name; return false; }
     }
@@ -507,6 +511,32 @@ void run_memtest(b2dp_ctx* ctx, const Flags& fl) {
     }
 }
 
+// -compute_test_at_start=1: run the tensor-core self-test on every GPU once, after open (and after the memtest) and
+// before the first registration.  A failed device stays latched Unhealthy, reported like a failed memtest.
+void run_compute_test(b2dp_ctx* ctx, const Flags& fl) {
+    b2dp_compute_test_opts o{};
+    o.duration_ms = fl.compute_test_ms;
+    o.fault_sm = -1;
+    if (fl.compute_test_at_start >= 2) o.flags |= B2DP_CT_EVEN_IF_BUSY;
+    b2dp_compute_test_result res[64];
+    int n = 0;
+    const int rc = b2dp_compute_test(ctx, -1, &o, res, 64, &n);
+    if (rc != B2DP_OK) {
+        logf("compute test at start not run: %s (%s)", b2dp_strerror(rc), b2dp_last_error(ctx));
+        return;
+    }
+    std::vector<b2dp_device> devs(n > 0 ? n : 1);
+    int nd = 0;
+    if (b2dp_enumerate(ctx, devs.data(), (int)devs.size(), &nd) != B2DP_OK) nd = 0;
+    for (int i = 0; i < n; ++i) {
+        const b2dp_compute_test_result& r = res[i];
+        logf("compute test %s: %s, flags 0x%x, SMs %d/%d, mismatches %llu/%llu/%llu, first bad SM %d, %.0f/%.0f/%.0f "
+             "TFLOP/s", r.device < nd ? devs[r.device].id : "?", r.healthy ? "Healthy" : "Unhealthy", r.flags,
+             r.sms_covered, r.sm_count, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
+             (unsigned long long)r.mismatches[2], r.first_bad_sm, r.tflops[0], r.tflops[1], r.tflops[2]);
+    }
+}
+
 }  // namespace
 
 int main(int argc, char** argv) {
@@ -538,6 +568,7 @@ int main(int argc, char** argv) {
     int rc = b2dp_open(fl.backend.c_str(), &ctx);
     if (rc != B2DP_OK) { logf("open %s: %s (%s)", fl.backend.c_str(), b2dp_strerror(rc), b2dp_last_error(nullptr)); return 1; }
     if (fl.memtest_at_start) run_memtest(ctx, fl);
+    if (fl.compute_test_at_start) run_compute_test(ctx, fl);
     char names[64][64];
     int n_res = 0;
     rc = b2dp_resource_list(ctx, fl.strategy.c_str(), names, 64, &n_res);  // main.go:141-146

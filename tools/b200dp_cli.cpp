@@ -7,7 +7,7 @@
 //       -Wl,-rpath,'$ORIGIN/../k8s-device-plugin_b200' -o tools/b200dp_cli
 //
 //   b200dp_cli <backend-uri> enumerate | health | cycle [steps [idle_ms]] | probe [steps] | resources <single|mixed>
-//                            | labels <csv> | alloc <size> | p2p | memtest [max_bytes]
+//                            | labels <csv> | alloc <size> | p2p | memtest [max_bytes] | compute_test [duration_ms]
 #include <algorithm>
 #include <chrono>
 #include <ctime>
@@ -148,6 +148,27 @@ int main(int argc, char** argv) {
                    r.n_segments, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
                    (unsigned long long)r.mismatches[2], (unsigned long long)r.mismatches[3], (long long)r.first_bad_word,
                    (unsigned long long)r.ecc_corrected, (unsigned long long)r.ecc_uncorrected, r.ms, r.gbs);
+            bad += !r.healthy;
+        }
+        b2dp_close(ctx);
+        return bad ? 1 : 0;
+    } else if (cmd == "compute_test") {  // one line per device; exit status 1 if any device is Unhealthy
+        b2dp_compute_test_opts co{};
+        co.duration_ms = argc > 3 ? (uint32_t)strtoul(argv[3], nullptr, 0) : 0;
+        co.fault_sm = -1;
+        std::vector<b2dp_compute_test_result> res(n ? n : 1);
+        int m = 0;
+        if ((rc = b2dp_compute_test(ctx, -1, &co, res.data(), (int)res.size(), &m)) != B2DP_OK)
+            return die(ctx, "b2dp_compute_test", rc);
+        int bad = 0;
+        for (int i = 0; i < m; ++i) {
+            const b2dp_compute_test_result& r = res[i];
+            printf("%s %s err=%d flags=0x%x sms=%d/%d nsmid=%d mismatches=%llu,%llu,%llu first_bad_sm=%d "
+                   "first_bad_format=%d first_bad_tile=%d ms=%.1f,%.1f,%.1f tflops_bf16=%.0f tflops_fp8=%.0f tops_int8=%.0f\n",
+                   devs[r.device].id, r.healthy ? "Healthy" : "Unhealthy", r.err, r.flags, r.sms_covered, r.sm_count,
+                   r.nsmid, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
+                   (unsigned long long)r.mismatches[2], r.first_bad_sm, r.first_bad_format, r.first_bad_tile, r.ms[0],
+                   r.ms[1], r.ms[2], r.tflops[0], r.tflops[1], r.tflops[2]);
             bad += !r.healthy;
         }
         b2dp_close(ctx);
