@@ -40,7 +40,7 @@
 
 namespace b2dp {
 
-// the kernel shapes (kTma*, kReg*) are defined next to the kernels in hbm_probe.cuh
+// the kernel shapes (kTma*, kQueue*, kReg*) are defined next to the kernels in hbm_probe.cuh
 constexpr unsigned long long kFloorMinBytes = 128ull << 20;  // a ring slot well above the 50 MB L2: the pass measures HBM, not the cache
 
 // bit b of (uint32(i) * K) summed over i < n_words, for the closed-form checksum
@@ -242,8 +242,8 @@ static void launch_probe(Gpu* g, unsigned long long n_vec, uint32_t variant, uin
         hbm_probe_r128<kRegThreads, kRegUnroll><<<grid > 0 ? grid : (int)g->sms * kRegCtasPerSm, kRegThreads, 0, g->stream>>>(
             src, dst, n_vec, seed, delta, g->ctl, g->out_d, seq);
     else
-        hbm_probe_tma<kTmaCW, kTmaTileVec, kTmaStages>
-            <<<grid > 0 ? grid : (int)g->sms * kTmaCtasPerSm, (kTmaCW + 1) * 32, kTmaSmem, g->stream>>>(
+        hbm_probe_queue<kQueueCW, kQueueTileVec, kQueueStages>
+            <<<grid > 0 ? grid : (int)g->sms * kQueueCtasPerSm, (kQueueCW + 2) * 32, kQueueSmem, g->stream>>>(
                 src, dst, n_vec, seed, delta, g->ctl, g->out_d, seq);
 }
 
@@ -606,6 +606,10 @@ int cuda_backend_open(const CudaConfig& cfg, CudaBackend** out, std::string& err
             TRY(cudaFuncSetAttribute(hbm_probe_tma<kTmaCW, kTmaTileVec, kTmaStages>,
                                      cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTmaSmem));
             TRY(cudaFuncSetAttribute(hbm_probe_tma<kTmaCW, kTmaTileVec, kTmaStages>,
+                                     cudaFuncAttributePreferredSharedMemoryCarveout, 100));
+            TRY(cudaFuncSetAttribute(hbm_probe_queue<kQueueCW, kQueueTileVec, kQueueStages>,
+                                     cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kQueueSmem));
+            TRY(cudaFuncSetAttribute(hbm_probe_queue<kQueueCW, kQueueTileVec, kQueueStages>,
                                      cudaFuncAttributePreferredSharedMemoryCarveout, 100));
             g->seed = 0x5EED0000u | (uint32_t)(seed_idx & 0xffff);  // SURVEY 8(d) config 2
             g->cur = 0;
@@ -1827,8 +1831,8 @@ int cuda_p2p_matrix(CudaBackend* be, const b2dp_p2p_opts* opts, float* gbs, int3
             for (int it = 0; it < iters + 1; ++it) {  // first iteration is a warm-up
                 const unsigned long long seq = ++g->seq;
                 cudaEventRecord(g->e0, g->stream);
-                // the same smem-staged kernel as the health probe, with a peer-mapped source: the bulk
-                // copies cross NVLink, verification happens on the receiving GPU
+                // the former health-probe kernel (smem-staged, tile t -> CTA t mod grid) with a peer-mapped
+                // source: the bulk copies cross NVLink, verification happens on the receiving GPU
                 hbm_probe_tma<kTmaCW, kTmaTileVec, kTmaStages>
                     <<<(int)g->sms * kTmaCtasPerSm, (kTmaCW + 1) * 32, kTmaSmem, g->stream>>>(
                         src, g->buf[g->next()], n_vec, seed, 0u, g->ctl, g->out_d, seq);

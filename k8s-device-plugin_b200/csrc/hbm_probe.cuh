@@ -41,6 +41,15 @@ constexpr int kTmaCtasPerSm = 2;    // 2 x 3 x 16 KiB = 96 KiB staged per SM
 constexpr size_t kTmaSmem = tma_smem_bytes(kTmaTileVec, kTmaStages);
 constexpr int kRegThreads = 512, kRegUnroll = 2, kRegCtasPerSm = 2;
 
+// Dynamic shared memory of one hbm_probe_queue CTA: the tile ring, its full/done/empty mbarriers and the tile of each slot.
+constexpr size_t queue_smem_bytes(int tile_vec, int stages) { return (size_t)stages * tile_vec * 16 + 4 * stages * 8; }
+// The health probe's kernel (hbm_probe_queue); hbm_probe_tma above stays the P2P and memtest shape.
+constexpr int kQueueCW = 4;           // verifier warps (plus a loader and a storer warp)
+constexpr int kQueueTileVec = 512;    // 8 KiB tiles
+constexpr int kQueueStages = 6;
+constexpr int kQueueCtasPerSm = 2;    // 2 x 6 x 8 KiB = 96 KiB staged per SM, as hbm_probe_tma
+constexpr size_t kQueueSmem = queue_smem_bytes(kQueueTileVec, kQueueStages);
+
 // Device-resident control block (one per GPU, zero-initialised once).
 struct ProbeCtl {
     unsigned long long checksum;      // running sum over this launch
@@ -48,7 +57,7 @@ struct ProbeCtl {
     unsigned long long first_bad;     // min word index with a mismatch (~0 = none)
     unsigned long long t_start_ns;    // min %globaltimer over CTAs
     unsigned int       done;          // CTA completion ticket
-    unsigned int       pad;
+    unsigned int       next_tile;     // hbm_probe_queue's tile queue (0 between launches)
 };
 
 // Result block; lives in pinned, device-mapped host memory so the last CTA
@@ -413,6 +422,116 @@ hbm_probe_tma(const uint4* __restrict__ src, uint4* __restrict__ dst, unsigned l
     }
 
     // ragged tail: vectors past the last full tile, register path
+    for (unsigned long long i = n_tiles * TILE_VEC + (unsigned long long)blockIdx.x * THREADS + threadIdx.x;
+         i < n_vec; i += (unsigned long long)gridDim.x * THREADS) {
+        uint4 v = ldg_na(src + i);
+        check4(v, i, seed, delta, a);
+        stg_na(dst + i, v);
+    }
+    finish<THREADS>(a, ctl, out, seq, t0);
+}
+
+// ===========================================================================
+// Variant QUEUE (the health probe's kernel): a TMA ring like hbm_probe_tma's, with two changes
+// that tools/probe_sweep --gap measured (profiles/README.md):
+//  * CTAs take tiles from a grid-wide queue (ctl->next_tile) instead of tile t -> CTA t mod grid.
+//    With a fixed split the CTAs of a full grid finish up to a third of a pass apart, and HBM idles
+//    while the slowest drain; from a queue, a CTA that streams faster simply takes more tiles.
+//  * Loads and stores are issued by different warps, so a refill never waits behind a store.
+// Roles:
+//   warp 0 lane 0 = loader : wait empty[s] -> claim a tile -> tile_of[s] = t -> bulk load into s
+//                            (no tile left: tile_of[s] = kNoTile, plain arrive on full[s], stop)
+//   warp 1 lane 0 = storer : wait full[s] -> wait done[s] -> bulk store s -> wait until it has read
+//                            s -> arrive empty[s]
+//   warps 2..CW+1 = verifiers: wait full[s] -> check4 + re-key their share in place -> arrive done[s]
+// The mbarrier arrive that publishes full[s] releases tile_of[s]; every reader waits on full[s].
+// Every CTA makes exactly one claim past the last tile, so n_tiles + gridDim.x claims are made per
+// launch and the CTA that gets the last one resets the queue for the next launch on the stream
+// (n_tiles + gridDim.x must stay below 2^32: 32 TiB of 8 KiB tiles).
+// The ragged tail (n_vec mod TILE_VEC vectors) is a static grid-stride register loop, as in hbm_probe_tma.
+// Dynamic smem = STAGES*TILE_VEC*16 + 4*STAGES*8.
+// ===========================================================================
+template <int CW, int TILE_VEC, int STAGES>
+__global__ void __launch_bounds__((CW + 2) * 32)
+hbm_probe_queue(const uint4* __restrict__ src, uint4* __restrict__ dst, unsigned long long n_vec,
+                uint32_t seed, uint32_t delta, ProbeCtl* ctl, ProbeOut* out, unsigned long long seq) {
+    constexpr int THREADS = (CW + 2) * 32;
+    constexpr int CT = CW * 32;  // verifier threads
+    static_assert(TILE_VEC % CT == 0, "tile must be a multiple of the verifier width");
+    static_assert(STAGES >= 2, "need >=2 stages");
+    constexpr int PER_THREAD = TILE_VEC / CT;
+    constexpr uint32_t TILE_BYTES = TILE_VEC * 16u;
+    constexpr unsigned long long kNoTile = ~0ull;
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    uint4* tiles = reinterpret_cast<uint4*>(smem_raw);
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem_raw + (size_t)STAGES * TILE_BYTES);
+    uint64_t* done = full + STAGES;
+    uint64_t* empty = done + STAGES;
+    unsigned long long* tile_of = reinterpret_cast<unsigned long long*>(empty + STAGES);
+
+    const unsigned long long t0 = globaltimer_ns();
+    const unsigned long long n_tiles = n_vec / TILE_VEC;
+
+    if (threadIdx.x == 0) {
+#pragma unroll
+        for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&done[s], CT); mbar_init(&empty[s], 1); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        fence_proxy_async_smem();
+    }
+    __syncthreads();
+
+    Acc a;
+    if (threadIdx.x == 0) {
+        unsigned long long t = atomicAdd(&ctl->next_tile, 1u);
+        for (unsigned long long k = 0;; ++k) {
+            const int slot = (int)(k % STAGES);
+            if (k >= STAGES) mbar_wait(&empty[slot], (uint32_t)((k / STAGES - 1) & 1));
+            if (t >= n_tiles) {
+                tile_of[slot] = kNoTile;
+                mbar_arrive(&full[slot]);
+                if (t == n_tiles + gridDim.x - 1) atomicExch(&ctl->next_tile, 0u);  // the launch's last claim
+                break;
+            }
+            tile_of[slot] = t;
+            mbar_expect_tx(&full[slot], TILE_BYTES);
+            bulk_g2s(tiles + (size_t)slot * TILE_VEC, src + t * TILE_VEC, TILE_BYTES, &full[slot]);
+            t = atomicAdd(&ctl->next_tile, 1u);  // the next claim travels while the ring is full
+        }
+    } else if (threadIdx.x == 32) {
+        for (unsigned long long k = 0;; ++k) {
+            const int slot = (int)(k % STAGES);
+            const uint32_t parity = (uint32_t)((k / STAGES) & 1);
+            mbar_wait(&full[slot], parity);
+            const unsigned long long t = tile_of[slot];
+            if (t == kNoTile) break;
+            mbar_wait(&done[slot], parity);
+            bulk_s2g(dst + t * TILE_VEC, tiles + (size_t)slot * TILE_VEC, TILE_BYTES);
+            bulk_commit();
+            bulk_wait_read<0>();  // the store no longer reads the slot: hand it back to the loader
+            mbar_arrive(&empty[slot]);
+        }
+        bulk_wait_all<0>();
+    } else if (threadIdx.x >= 64) {
+        const int ct = threadIdx.x - 64;
+        for (unsigned long long k = 0;; ++k) {
+            const int slot = (int)(k % STAGES);
+            mbar_wait(&full[slot], (uint32_t)((k / STAGES) & 1));
+            const unsigned long long t = tile_of[slot];
+            if (t == kNoTile) break;
+            uint4* tile = tiles + (size_t)slot * TILE_VEC;
+            uint4 v[PER_THREAD];
+#pragma unroll
+            for (int u = 0; u < PER_THREAD; ++u) v[u] = tile[ct + u * CT];
+#pragma unroll
+            for (int u = 0; u < PER_THREAD; ++u) {
+                check4(v[u], t * TILE_VEC + ct + u * CT, seed, delta, a);
+                tile[ct + u * CT] = v[u];
+            }
+            fence_proxy_async_smem();
+            mbar_arrive(&done[slot]);
+        }
+    }
+
     for (unsigned long long i = n_tiles * TILE_VEC + (unsigned long long)blockIdx.x * THREADS + threadIdx.x;
          i < n_vec; i += (unsigned long long)gridDim.x * THREADS) {
         uint4 v = ldg_na(src + i);
