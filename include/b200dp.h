@@ -270,8 +270,8 @@ typedef struct b2dp_probe_result {
                                       last b2dp_probe_reset) => Unhealthy, sticky */
 #define B2DP_RES_MEMTEST 0x200u    /* a b2dp_memtest of this device failed or timed out since open (or the last
                                       b2dp_probe_reset) => Unhealthy, sticky */
-#define B2DP_RES_COMPUTE 0x400u    /* a b2dp_compute_test of this device failed or timed out since open (or the last
-                                      b2dp_probe_reset) => Unhealthy, sticky */
+#define B2DP_RES_COMPUTE 0x400u    /* a compute or FP self-test (b2dp_compute_test, b2dp_fp_test) of this device failed
+                                      or timed out since open (or the last b2dp_probe_reset) => Unhealthy, sticky */
 
 /* Replaces the exporter round trip getGPUHealth (exporter/health.go:42-82) and the evidence behind simpleHealthCheck
  * (plugin.go:161-206): launch the probe on every GPU of the context concurrently (one worker thread + stream per
@@ -283,7 +283,7 @@ B2DP_API int b2dp_probe_health(b2dp_ctx *ctx, const b2dp_probe_opts *opts, b2dp_
  * event numbered `mask` for `device` (seen by contexts opened with xid=1).  The reference has no equivalent. */
 B2DP_API int b2dp_probe_inject_fault(b2dp_ctx *ctx, int device, uint64_t word_index, uint32_t mask);
 /* Re-fill the probe buffers of `device` (-1 = all) with a clean pattern; also clears a latched Xid, a latched memtest
- * failure and a latched compute-test failure. */
+ * failure and a latched compute- or FP-test failure. */
 B2DP_API int b2dp_probe_reset(b2dp_ctx *ctx, int device);
 /* Set the bandwidth ceiling (gbs_ref) of `device` (-1 = all) the fractional floor refers to, e.g. to the site's measured
  * HBM peak; gbs_ref <= 0 restores the device's own calibration.  Also how tests move a device across the 0.8 line. */
@@ -407,6 +407,25 @@ typedef struct b2dp_compute_test_result {
  * unless B2DP_CT_EVEN_IF_BUSY.  cuda: backend with the in-process probe only; B2DP_E_UNSUPPORTED otherwise. */
 B2DP_API int b2dp_compute_test(b2dp_ctx *ctx, int device, const b2dp_compute_test_opts *opts,
                                b2dp_compute_test_result *out, int cap, int *n);
+
+/* ---- on-demand FP32 / FP64 self-test (same opts, result and latch as the tensor-core self-test) ---- */
+#define B2DP_FT_FP32 0             /* b2dp_fp_test's format index of mismatches[] / ms[] / tflops[] / first_bad_format */
+#define B2DP_FT_FP64 1
+#define B2DP_FT_DMMA 2
+
+/* An on-demand check of the SMs' FP32 FMA units, FP64 FMA units and FP64 tensor cores on `device` (-1 = every GPU,
+ * concurrently on their workers): evidence behind the per-GPU verdict the exporter round trip supplies in the reference
+ * (exporter/health.go:42-82), merged the same way (exporter/health.go:86-106) through the sticky B2DP_RES_COMPUTE bit.
+ * Per GPU and per format one launch of fp_selftest.cuh fills every SM for duration_ms with: independent fma.rn.f32
+ * (FFMA) and fma.rn.f64 (DFMA) on full-mantissa random operands plus crafted ties, cancellations, subnormal results,
+ * signed zeros and sticky-bit cases; and mma.sync m16n8k16 .f64 (DMMA) on scaled integer operands whose sums stay
+ * exact.  Every result is compared bit for bit with the host's IEEE 754 result (std::fmaf / std::fma, or the exact
+ * integer product).  The result struct is b2dp_compute_test_result with its per-format arrays indexed by B2DP_FT_*;
+ * tflops[] counts 2 FLOPs per FMA or multiply-add.  Healthy, latching, the probe lock, the busy skip, the deadline and
+ * the release of every allocation are exactly b2dp_compute_test's.  cuda: backend with the in-process probe only;
+ * B2DP_E_UNSUPPORTED otherwise. */
+B2DP_API int b2dp_fp_test(b2dp_ctx *ctx, int device, const b2dp_compute_test_opts *opts, b2dp_compute_test_result *out,
+                          int cap, int *n);
 
 /* exporter/health.go:86-106 PopulatePerGPUDHealth(devs, defaultHealth) merge rule.
  * have_source = 0 reproduces "exporter socket absent / RPC failed" (every device gets the

@@ -57,12 +57,12 @@ class ComputeTestResult:
     nsmid: int
     sms_covered: int               # SM ids on which every format ran at least one CTA
     bad_sm_mask: List[int]         # 4 x 64 bits over %smid
-    mismatches: List[int]          # per format: BF16, FP8, INT8
+    mismatches: List[int]          # per format: BF16, FP8, INT8 (fp_test: FP32, FP64, DMMA)
     first_bad_sm: int
     first_bad_format: int
     first_bad_tile: int
     ms: List[float]
-    tflops: List[float]            # 2 M N K x result tiles compared / ms (TOPS for INT8)
+    tflops: List[float]            # 2 M N K x result tiles compared / ms (TOPS for INT8; fp_test: 2 x FMAs / ms)
 
     def bad_sms(self) -> List[int]:
         return [s for s in range(256) if (self.bad_sm_mask[s // 64] >> (s % 64)) & 1]
@@ -221,6 +221,20 @@ class Context:
         opts = N.ComputeTestOpts(duration_ms, timeout_ms, N.CT_EVEN_IF_BUSY if even_if_busy else 0, fault_sm, fault_mask, 0)
         rc, arr, n = N.grow_call(lambda cap: (N.ComputeTestResult * cap)(),
                                  lambda a, cap, pn: N.lib.b2dp_compute_test(self._h, device, C.byref(opts), a, cap, pn))
+        N.check(rc, self._h)
+        return [ComputeTestResult(r.device, bool(r.healthy), r.err, r.flags, r.seed, r.sm_count, r.nsmid, r.sms_covered,
+                                  list(r.bad_sm_mask), list(r.mismatches), r.first_bad_sm, r.first_bad_format,
+                                  r.first_bad_tile, list(r.ms), list(r.tflops)) for r in arr[:n]]
+
+    def fp_test(self, device: int = -1, duration_ms: int = 0, timeout_ms: int = 0, even_if_busy: bool = False,
+                fault_sm: int = -1, fault_mask: int = 0) -> List[ComputeTestResult]:
+        """On-demand FP32 / FP64 self-test of `device` (-1 = every GPU, b2dp_fp_test): FFMA, DFMA and DMMA on every SM
+        for duration_ms each (0 = 1000), every result compared bit for bit with the host's IEEE 754 result.  The
+        per-format lists are indexed by FT_FP32, FT_FP64, FT_DMMA.  A failure is latched like compute_test()'s
+        (RES_COMPUTE until probe_reset()); fault_sm / fault_mask flips bits of one result on the SM with that %smid."""
+        opts = N.ComputeTestOpts(duration_ms, timeout_ms, N.CT_EVEN_IF_BUSY if even_if_busy else 0, fault_sm, fault_mask, 0)
+        rc, arr, n = N.grow_call(lambda cap: (N.ComputeTestResult * cap)(),
+                                 lambda a, cap, pn: N.lib.b2dp_fp_test(self._h, device, C.byref(opts), a, cap, pn))
         N.check(rc, self._h)
         return [ComputeTestResult(r.device, bool(r.healthy), r.err, r.flags, r.seed, r.sm_count, r.nsmid, r.sms_covered,
                                   list(r.bad_sm_mask), list(r.mismatches), r.first_bad_sm, r.first_bad_format,

@@ -35,6 +35,7 @@
 #include "memtest_math.hpp"
 #include "nvml_dyn.hpp"
 #include "pattern_math.hpp"
+#include "fp_selftest.cuh"
 #include "tc_selftest.cuh"
 #include "units_backend.hpp"
 
@@ -102,7 +103,7 @@ struct Gpu {
     bool xid_registered = false;
     std::atomic<unsigned long long> xid_fault{0};  // first critical Xid seen on this device (sticky, like a real fault)
     std::atomic<bool> memtest_fault{false};        // a b2dp_memtest failed or timed out (sticky until b2dp_probe_reset)
-    std::atomic<bool> compute_fault{false};        // a b2dp_compute_test failed or timed out (likewise)
+    std::atomic<bool> compute_fault{false};        // a b2dp_compute_test or b2dp_fp_test failed or timed out (likewise)
     int last_healthy = 1;
     // worker
     std::thread th;
@@ -1570,20 +1571,77 @@ static int cuda_memtest(CudaBackend* be, int device, const b2dp_memtest_opts* op
     return B2DP_OK;
 }
 
-// ---- on-demand tensor-core self-test (b2dp_compute_test) -------------------------------------------------------
-// One launch of tc_selftest.cuh per format on one GPU, on that GPU's worker.  The host builds every operand image and
-// every comparison value itself (compute_test_math.hpp): a health test must not ask the device under test for its own
-// reference values.  Every allocation is released before the job ends, whatever happened.
+// ---- on-demand compute self-tests (b2dp_compute_test, b2dp_fp_test) -----------------------------------------------
+// One launch per format on one GPU, on that GPU's worker: tc_selftest.cuh (tensor cores: BF16, FP8, INT8) or
+// fp_selftest.cuh (FP32 FMA, FP64 FMA, FP64 tensor cores).  The host builds every operand table and every comparison
+// value itself (compute_test_math.hpp, fp_test_math.hpp): a health test must not ask the device under test for its own
+// reference values.  Both tests share this driver -- grid sizing, records, tally, deadline, busy skip and the release
+// of every allocation before the job ends, whatever happened -- through a DiagSuite.
 constexpr uint32_t kComputeTestDefaultMs = 1000;
 
 using CtKernel = void (*)(const uint8_t*, const uint32_t*, unsigned long long, int, uint32_t, CtRecord*,
                           unsigned long long, uint32_t*);
+
+// The host's inputs of one launch per format: kCtTiles tables of table_bytes[f] and [kCtTiles][kCtThreads] checks.
+struct DiagTables {
+    std::vector<uint8_t> tables[kCtFormats];
+    std::vector<uint32_t> checks[kCtFormats];
+};
+
+struct DiagSuite {
+    const char* log_name;                      // "compute test" / "FP test"
+    const char* kernel_name;                   // for a CUDA error
+    const char* format_names;                  // "bf16/fp8/int8" / "fp32/fp64/dmma" in the log line
+    const CtKernel* kernels;                   // product instantiation per format
+    const uint32_t* smem;                      // dynamic shared memory per format
+    const uint32_t* table_bytes;               // bytes of one tile's table per format
+    void (*build_tile)(uint32_t seed, int fmt, int tile, uint8_t* table, uint32_t* check);
+    double (*macs_per_tile)(int fmt);          // multiply-adds of one comparison
+    bool per_device_seed;                      // seed ^ (device << 16) per GPU, tables built on each worker; else one
+                                               // seed and one set of tables per call
+};
+
+static void ct_suite_tile(uint32_t seed, int fmt, int tile, uint8_t* table, uint32_t* check) {
+    CtTile t;
+    ct_build_tile(seed, fmt, tile, t);
+    memcpy(table, t.image.data(), t.image.size());
+    memcpy(check, t.check, sizeof t.check);
+}
+static void ft_suite_tile(uint32_t seed, int fmt, int tile, uint8_t* table, uint32_t* check) {
+    FtTile t;
+    ft_build_tile(seed, fmt, tile, t);
+    memcpy(table, t.table.data(), t.table.size());
+    memcpy(check, t.check, sizeof t.check);
+}
+
 static const CtKernel kCtKernels[kCtFormats] = {tc_selftest<CT_BF16, false>, tc_selftest<CT_FP8, false>,
                                                 tc_selftest<CT_INT8, false>};
 static const uint32_t kCtSmem[kCtFormats] = {CtShape<CT_BF16>::SMEM, CtShape<CT_FP8>::SMEM, CtShape<CT_INT8>::SMEM};
+static const CtKernel kFtKernels[kFtFormats] = {fp_selftest<FT_FP32, false>, fp_selftest<FT_FP64, false>,
+                                                fp_selftest<FT_DMMA, false>};
+static const uint32_t kFtSmem[kFtFormats] = {0, 0, 0};
+static const uint32_t kFtTableBytes[kFtFormats] = {ft_table_bytes(FT_FP32), ft_table_bytes(FT_FP64),
+                                                   ft_table_bytes(FT_DMMA)};
+static const DiagSuite kTensorSuite = {"compute test", "tc_selftest", "bf16/fp8/int8", kCtKernels, kCtSmem, kCtSmem,
+                                       ct_suite_tile, ct_macs_per_tile, true};
+static const DiagSuite kFpSuite = {"FP test", "fp_selftest", "fp32/fp64/dmma", kFtKernels, kFtSmem, kFtTableBytes,
+                                   ft_suite_tile, ft_macs_per_tile, false};
 
-static void compute_test_one(Gpu* g, const b2dp_compute_test_opts& o, uint32_t duration_ms, uint32_t timeout_ms,
-                             b2dp_compute_test_result* r, std::string* err) {
+static std::shared_ptr<DiagTables> diag_build_tables(const DiagSuite& su, uint32_t seed) {
+    auto t = std::make_shared<DiagTables>();
+    for (int f = 0; f < kCtFormats; ++f) {
+        t->tables[f].resize((size_t)kCtTiles * su.table_bytes[f]);
+        t->checks[f].resize((size_t)kCtTiles * kCtThreads);
+        for (int tile = 0; tile < kCtTiles; ++tile)
+            su.build_tile(seed, f, tile, t->tables[f].data() + (size_t)tile * su.table_bytes[f],
+                          t->checks[f].data() + (size_t)tile * kCtThreads);
+    }
+    return t;
+}
+
+static void compute_test_one(const DiagSuite& su, Gpu* g, const b2dp_compute_test_opts& o, uint32_t duration_ms,
+                             uint32_t timeout_ms, std::shared_ptr<const DiagTables> tabs, b2dp_compute_test_result* r,
+                             std::string* err) {
     uint8_t* img[kCtFormats] = {};
     uint32_t* chk[kCtFormats] = {};
     CtRecord* rec_h = nullptr;
@@ -1607,35 +1665,30 @@ static void compute_test_one(Gpu* g, const b2dp_compute_test_opts& o, uint32_t d
         probe_flush(g);  // an armed heartbeat pass must not run underneath
         int grid[kCtFormats], off[kCtFormats + 1] = {0};
         for (int f = 0; f < kCtFormats; ++f) {
-            CT_TRY(cudaFuncSetAttribute(kCtKernels[f], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kCtSmem[f]));
-            CT_TRY(cudaFuncSetAttribute(kCtKernels[f], cudaFuncAttributePreferredSharedMemoryCarveout, 100));
+            CT_TRY(cudaFuncSetAttribute(su.kernels[f], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)su.smem[f]));
+            CT_TRY(cudaFuncSetAttribute(su.kernels[f], cudaFuncAttributePreferredSharedMemoryCarveout, 100));
             int per_sm = 0;
-            CT_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kCtKernels[f], kCtThreads, kCtSmem[f]));
+            CT_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, su.kernels[f], kCtThreads, su.smem[f]));
             grid[f] = (int)g->sms * (per_sm > 0 ? per_sm : 1);  // every CTA resident at once
             off[f + 1] = off[f] + grid[f];
         }
         CT_TRY(cudaHostAlloc(&rec_h, (size_t)off[kCtFormats] * sizeof(CtRecord), cudaHostAllocMapped));
         memset(rec_h, 0, (size_t)off[kCtFormats] * sizeof(CtRecord));
         CT_TRY(cudaHostGetDevicePointer(&rec_d, rec_h, 0));
+        if (!tabs) tabs = diag_build_tables(su, r->seed);
         for (int f = 0; f < kCtFormats; ++f) {
-            std::vector<uint8_t> images((size_t)kCtTiles * kCtSmem[f]);
-            std::vector<uint32_t> checks((size_t)kCtTiles * kCtThreads);
-            CtTile t;
-            for (int tile = 0; tile < kCtTiles; ++tile) {
-                ct_build_tile(r->seed, f, tile, t);
-                memcpy(images.data() + (size_t)tile * kCtSmem[f], t.image.data(), kCtSmem[f]);
-                memcpy(checks.data() + (size_t)tile * kCtThreads, t.check, sizeof t.check);
-            }
-            CT_TRY(cudaMalloc(&img[f], images.size()));
+            const std::vector<uint8_t>& tables = tabs->tables[f];
+            const std::vector<uint32_t>& checks = tabs->checks[f];
+            CT_TRY(cudaMalloc(&img[f], tables.size()));
             CT_TRY(cudaMalloc(&chk[f], checks.size() * sizeof(uint32_t)));
-            CT_TRY(cudaMemcpy(img[f], images.data(), images.size(), cudaMemcpyHostToDevice));
+            CT_TRY(cudaMemcpy(img[f], tables.data(), tables.size(), cudaMemcpyHostToDevice));
             CT_TRY(cudaMemcpy(chk[f], checks.data(), checks.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
         }
         for (cudaEvent_t& e : ev) CT_TRY(cudaEventCreate(&e));
 
         CT_TRY(cudaEventRecord(ev[0], g->stream));
         for (int f = 0; f < kCtFormats; ++f) {
-            kCtKernels[f]<<<grid[f], kCtThreads, kCtSmem[f], g->stream>>>(
+            su.kernels[f]<<<grid[f], kCtThreads, su.smem[f], g->stream>>>(
                 img[f], chk[f], (unsigned long long)duration_ms * 1000000ull, o.fault_sm, o.fault_mask, rec_d + off[f],
                 (unsigned long long)(f + 1), nullptr);
             CT_TRY(cudaGetLastError());
@@ -1645,7 +1698,7 @@ static void compute_test_one(Gpu* g, const b2dp_compute_test_opts& o, uint32_t d
         for (;;) {
             const cudaError_t q = cudaEventQuery(ev[kCtFormats]);
             if (q == cudaSuccess) break;
-            if (q != cudaErrorNotReady) { ce = q; where = "tc_selftest"; goto done; }
+            if (q != cudaErrorNotReady) { ce = q; where = su.kernel_name; goto done; }
             if (std::chrono::steady_clock::now() > deadline) { timed_out = true; break; }
             std::this_thread::sleep_for(std::chrono::milliseconds(1));
         }
@@ -1681,7 +1734,7 @@ static void compute_test_one(Gpu* g, const b2dp_compute_test_opts& o, uint32_t d
                 r->first_bad_sm = bad_sm;
                 r->first_bad_tile = bad_tile;
             }
-            if (r->ms[f] > 0) r->tflops[f] = (float)(2.0 * ct_macs_per_tile(f) * (double)compared / r->ms[f] * 1e-9);
+            if (r->ms[f] > 0) r->tflops[f] = (float)(2.0 * su.macs_per_tile(f) * (double)compared / r->ms[f] * 1e-9);
         }
         for (int s = 0; s < kCtMaxSmId; ++s) r->sms_covered += seen[0][s] && seen[1][s] && seen[2][s];
         if (r->sms_covered < r->sm_count) r->flags |= B2DP_CT_PARTIAL_COVERAGE;
@@ -1701,10 +1754,11 @@ done:
     }
 }
 
-static int cuda_compute_test(CudaBackend* be, int device, const b2dp_compute_test_opts* opts,
-                             std::vector<b2dp_compute_test_result>& out, std::string& err) {
+static int cuda_diag_test(const DiagSuite& su, CudaBackend* be, int device, const b2dp_compute_test_opts* opts,
+                          std::vector<b2dp_compute_test_result>& out, std::string& err) {
     if (be->units) {
-        err = "the compute self-test runs in-process only (not with probe=helpers / probe=off / MIG)";
+        err = std::string("the ") + (su.per_device_seed ? "compute self-test" : "FP self-test") +
+              " runs in-process only (not with probe=helpers / probe=off / MIG)";
         return B2DP_E_UNSUPPORTED;
     }
     if (device < -1 || device >= (int)be->gpus.size()) { err = "device index out of range"; return B2DP_E_INVAL; }
@@ -1715,6 +1769,8 @@ static int cuda_compute_test(CudaBackend* be, int device, const b2dp_compute_tes
     {
         std::lock_guard<std::mutex> pl(be->probe_mu);  // a heartbeat waits for a running self-test
         const uint32_t seed = (uint32_t)std::chrono::steady_clock::now().time_since_epoch().count() * kPatternMul;
+        // one seed for every GPU: the tables are built once, here, and shared by the workers
+        std::shared_ptr<const DiagTables> shared = su.per_device_seed ? nullptr : diag_build_tables(su, seed);
         std::vector<size_t> sel;
         for (size_t i = 0; i < be->gpus.size(); ++i) if (device < 0 || (int)i == device) sel.push_back(i);
         out.assign(sel.size(), b2dp_compute_test_result{});
@@ -1724,7 +1780,7 @@ static int cuda_compute_test(CudaBackend* be, int device, const b2dp_compute_tes
             Gpu* g = be->gpus[sel[k]].get();
             b2dp_compute_test_result* r = &out[k];
             r->device = (int32_t)sel[k];
-            r->seed = seed ^ ((uint32_t)sel[k] << 16);
+            r->seed = su.per_device_seed ? seed ^ ((uint32_t)sel[k] << 16) : seed;
             r->sm_count = (int32_t)g->sms;
             r->first_bad_sm = r->first_bad_format = r->first_bad_tile = -1;
             if (g->broken) { r->err = B2DP_E_CUDA; errs[k] = g->broken_reason + " on " + g->dev.id; continue; }
@@ -1734,7 +1790,10 @@ static int cuda_compute_test(CudaBackend* be, int device, const b2dp_compute_tes
                 continue;
             }
             std::string* e = &errs[k];
-            cs[k] = post(g, [g, o, duration_ms, timeout_ms, r, e] { compute_test_one(g, o, duration_ms, timeout_ms, r, e); });
+            const DiagSuite* sp = &su;
+            cs[k] = post(g, [sp, g, o, duration_ms, timeout_ms, shared, r, e] {
+                compute_test_one(*sp, g, o, duration_ms, timeout_ms, shared, r, e);
+            });
         }
         for (size_t k = 0; k < sel.size(); ++k) {
             if (cs[k]) cs[k]->wait();  // no deadline here: the buffers must be released before the call returns
@@ -1743,9 +1802,9 @@ static int cuda_compute_test(CudaBackend* be, int device, const b2dp_compute_tes
             Gpu* g = be->gpus[sel[k]].get();
             const b2dp_compute_test_result& r = out[k];
             if (!r.healthy) { g->compute_fault.store(true); latched = true; }
-            logf(r.healthy ? 0 : 2, "%s compute test: %s, SMs %d/%d, mismatches bf16/fp8/int8 %llu/%llu/%llu, first bad SM %d "
-                 "format %d tile %d, %.1f/%.1f/%.1f ms, %.0f/%.0f/%.0f TFLOP/s%s", g->dev.id.c_str(),
-                 r.healthy ? "Healthy" : "Unhealthy (latched)", r.sms_covered, r.sm_count,
+            logf(r.healthy ? 0 : 2, "%s %s: %s, SMs %d/%d, mismatches %s %llu/%llu/%llu, first bad SM %d "
+                 "format %d tile %d, %.1f/%.1f/%.1f ms, %.0f/%.0f/%.0f TFLOP/s%s", g->dev.id.c_str(), su.log_name,
+                 r.healthy ? "Healthy" : "Unhealthy (latched)", r.sms_covered, r.sm_count, su.format_names,
                  (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
                  (unsigned long long)r.mismatches[2], r.first_bad_sm, r.first_bad_format, r.first_bad_tile, r.ms[0],
                  r.ms[1], r.ms[2], r.tflops[0], r.tflops[1], r.tflops[2], r.err == B2DP_E_TIMEOUT ? ", timed out" : "");
@@ -1756,6 +1815,16 @@ static int cuda_compute_test(CudaBackend* be, int device, const b2dp_compute_tes
     return B2DP_OK;
 }
 
+static int cuda_compute_test(CudaBackend* be, int device, const b2dp_compute_test_opts* opts,
+                             std::vector<b2dp_compute_test_result>& out, std::string& err) {
+    return cuda_diag_test(kTensorSuite, be, device, opts, out, err);
+}
+
+static int cuda_fp_test(CudaBackend* be, int device, const b2dp_compute_test_opts* opts,
+                        std::vector<b2dp_compute_test_result>& out, std::string& err) {
+    return cuda_diag_test(kFpSuite, be, device, opts, out, err);
+}
+
 static bool cuda_diag_latched(CudaBackend* be) {
     for (auto& g : be->gpus)
         if (g->memtest_fault.load() || g->compute_fault.load()) return true;
@@ -1764,7 +1833,7 @@ static bool cuda_diag_latched(CudaBackend* be) {
 
 // registered when the library is loaded, before any entry point can run (internal.hpp DiagHooks)
 [[maybe_unused]] static const bool kDiagRegistered = [] {
-    diag_hooks() = DiagHooks{cuda_memtest, cuda_compute_test, cuda_diag_latched};
+    diag_hooks() = DiagHooks{cuda_memtest, cuda_compute_test, cuda_fp_test, cuda_diag_latched};
     return true;
 }();
 

@@ -143,9 +143,10 @@ bool cuda_device_paths(CudaBackend*, const std::string& id, std::vector<std::str
 // xid=1: called (from a backend thread, or from b2dp_probe_inject_fault) when a device-level Xid has been latched
 void cuda_set_health_event_callback(CudaBackend*, std::function<void()> fn);
 
-// The on-demand diagnostics (the memory test and the compute self-test) are optional capabilities of the cuda backend:
+// The on-demand diagnostics (the memory test and the compute and FP self-tests) are optional capabilities of the cuda backend:
 // a build of the library whose backend has none (the CPU-only build of ctx.cpp the sanitizer tests link against a
-// stand-in backend) simply leaves these null, and b2dp_memtest / b2dp_compute_test then return B2DP_E_UNSUPPORTED.
+// stand-in backend) simply leaves these null, and b2dp_memtest / b2dp_compute_test / b2dp_fp_test then return
+// B2DP_E_UNSUPPORTED.
 // cuda_backend.cu fills them in during static initialisation.
 struct DiagHooks {
     // b2dp_memtest on `device` (-1 = all); B2DP_E_UNSUPPORTED without the in-process probe
@@ -154,7 +155,10 @@ struct DiagHooks {
     // b2dp_compute_test on `device` (-1 = all); B2DP_E_UNSUPPORTED without the in-process probe
     int (*compute_test)(CudaBackend*, int device, const b2dp_compute_test_opts* opts,
                         std::vector<b2dp_compute_test_result>& out, std::string& err) = nullptr;
-    // true while any device carries a latched memtest or compute-test failure (cleared by b2dp_probe_reset)
+    // b2dp_fp_test on `device` (-1 = all); B2DP_E_UNSUPPORTED without the in-process probe
+    int (*fp_test)(CudaBackend*, int device, const b2dp_compute_test_opts* opts,
+                   std::vector<b2dp_compute_test_result>& out, std::string& err) = nullptr;
+    // true while any device carries a latched memtest, compute-test or FP-test failure (cleared by b2dp_probe_reset)
     bool (*latched)(CudaBackend*) = nullptr;
 };
 DiagHooks& diag_hooks();  // ctx.cpp
