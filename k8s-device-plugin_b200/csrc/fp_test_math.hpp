@@ -46,12 +46,14 @@ enum FtClass {
     FT_ZERO_POS,       // x * a = -b exactly: +0
     FT_ZERO_NEG,       // x * a = -0 and b = -0: -0
     FT_STICKY,         // |b| > 2^M |x * a| and |x * a| in (ulp(b) / 2, ulp(b)): only the sticky bit says "round up"
+    FT_SUB_OPERAND,    // a subnormal (top stored bit set), b normal in [2^EMIN, 2^(EMIN + 4)): every x_i * a moves the
+                       // result off b, so a unit that reads a subnormal multiplicand as 0 gets all 8 results wrong
     kFtClasses
 };
 inline int ft_class_slot(int c, int t) { return (2 * c + t) % kFtAB; }
 inline int ft_class_x(int c) {
     // x_0 has an odd significand, x_1 an even one that is not a power of two, x_2 the exponent -8, x_3 is random
-    static const int x[kFtClasses] = {0, 1, 0, 2, 1, 3, 0};
+    static const int x[kFtClasses] = {0, 1, 0, 2, 1, 3, 0, 3};
     return x[c];
 }
 
@@ -63,7 +65,8 @@ struct FtBin {
 constexpr FtBin kFtBin32 = {32, 23, 127, -126, 16, 40, 28};
 constexpr FtBin kFtBin64 = {64, 52, 1023, -1022, 16, 300, 60};
 inline const FtBin& ft_bin(int fmt) { return fmt == FT_FP32 ? kFtBin32 : kFtBin64; }
-// every random or crafted operand stays normal (the subnormal class's b excepted) and every product below overflow
+// every random or crafted operand stays normal (the subnormal class's b and the subnormal-operand class's a excepted)
+// and every product below overflow
 static_assert(kFtBin32.x_exp + kFtBin32.a_exp + kFtBin32.M + 2 < 127 &&
               kFtBin32.a_exp + kFtBin32.b_spread < 127 && -(kFtBin32.x_exp + kFtBin32.a_exp + kFtBin32.M + 1) > -126,
               "FP32 operand exponents stay in the normal range");
@@ -195,6 +198,10 @@ inline void ft_fma_thread(uint32_t seed, int fmt, int tile, int t, FtFmaOperands
             case FT_STICKY:  // ulp(b) = 2^(q + 1); b's significand even, so a lost sticky bit would round to b
                 o.a[k] = pow2;
                 o.b[k] = ft_make(f, sb, q + f.M + 1, o.b[k] & ~1ull);
+                break;
+            case FT_SUB_OPERAND:  // |x_i * a| >= 2^(EMIN - 17) > ulp(b) / 2 = 2^(e(b) - M - 1) for every x_i
+                o.a[k] = ft_make(f, sa, f.EMIN - 1, o.a[k] | 1ull << (f.M - 1));
+                o.b[k] = ft_make(f, sb, ct_uniform(ft_draw(key, t, kFtX + kFtAB + k, 3), f.EMIN, f.EMIN + 3), o.b[k]);
                 break;
         }
     }

@@ -31,8 +31,8 @@ M32 = 0xFFFFFFFF
 BIN = {FP32: (32, 23, 127, -126, 16, 40, 28), FP64: (64, 52, 1023, -1022, 16, 300, 60)}
 CANCEL_BITS = {FP32: 20, FP64: 40}
 SUBNORMAL_X_EXP = -8
-CLASSES = ("tie_away", "tie_toward", "cancel", "subnormal", "zero_pos", "zero_neg", "sticky")
-CLASS_X = (0, 1, 0, 2, 1, 3, 0)
+CLASSES = ("tie_away", "tie_toward", "cancel", "subnormal", "zero_pos", "zero_neg", "sticky", "subnormal_operand")
+CLASS_X = (0, 1, 0, 2, 1, 3, 0, 3)
 
 DMMA_STEPS, DMMA_SETS, DMMA_K = 4, 4, 64
 DMMA_MAX = 11863283
@@ -67,15 +67,28 @@ def make(fmt, sign, e, mant):
     return sign << (W - 1) | (e + BIAS) << M | (mant & ((1 << M) - 1))
 
 
+class NaNResult(ValueError):
+    """An operation whose IEEE 754 result is NaN (or a NaN operand): its payload is unspecified, so no test uses one."""
+
+
 def decode(fmt, bits):
-    """(sign, N, E): the value is (-1)^sign * N * 2^E with N a non-negative integer."""
+    """(sign, N, E): the value is (-1)^sign * N * 2^E with N a non-negative integer; N is None for an infinity."""
     W, M, BIAS, EMIN = BIN[fmt][:4]
     sign = bits >> (W - 1) & 1
     be = bits >> M & ((1 << (W - M - 1)) - 1)
     mant = bits & ((1 << M) - 1)
     if be == 0:
         return sign, mant, EMIN - M
+    if be == (1 << (W - M - 1)) - 1:
+        if mant:
+            raise NaNResult("NaN operand 0x%x" % bits)
+        return sign, None, 0
     return sign, mant | 1 << M, be - BIAS - M
+
+
+def inf(fmt, sign):
+    W, M = BIN[fmt][:2]
+    return sign << (W - 1) | ((1 << (W - M - 1)) - 1) << M
 
 
 def exponent(fmt, bits):
@@ -83,35 +96,73 @@ def exponent(fmt, bits):
     return (bits >> M & ((1 << (W - M - 1)) - 1)) - BIAS
 
 
-def round_rne(fmt, sign, N, E, ties_away=False):
-    """Bits of (-1)^sign N 2^E (N > 0) rounded to nearest-even, and how: (bits, tie, rounded_up).  ties_away rounds
-    ties away from zero instead (a wrong rule, for tests that need one)."""
+# Rounding rules: IEEE 754's round to nearest, ties to even ("rne"), and wrong ones for the fault models of
+# tests/fp_test_faults.py: ties away from zero, ties toward zero, truncation, and "no_sticky", which sees only the round
+# bit (a set round bit is taken for a tie).
+def round_shift(N, sh, mode="rne"):
+    """(N >> sh rounded by `mode`, tie, rounded_up) for sh >= 1."""
+    mant, rem, half = N >> sh, N & ((1 << sh) - 1), 1 << (sh - 1)
+    tie = rem == half
+    if mode == "rne":
+        up = rem > half or (tie and mant & 1 == 1)
+    elif mode == "ties_away":
+        up = rem >= half
+    elif mode == "ties_toward_zero":
+        up = rem > half
+    elif mode == "truncate":
+        up = False
+    elif mode == "no_sticky":
+        up = rem & half != 0 and mant & 1 == 1
+    else:
+        raise ValueError(mode)
+    return mant + up, tie, up
+
+
+def round_rne(fmt, sign, N, E, ties_away=False, mode="rne"):
+    """Bits of (-1)^sign N 2^E (N > 0) rounded to nearest-even, and how: (bits, tie, rounded_up).  A value whose
+    rounded magnitude exceeds the largest finite one is an infinity (a truncating rule gives the largest finite value).
+    ties_away, or another `mode` of round_shift, rounds by a wrong rule instead (for tests that need one)."""
     W, M, BIAS, EMIN = BIN[fmt][:4]
+    mode = "ties_away" if ties_away else mode
     lead = E + N.bit_length() - 1
     q = max(lead - M, EMIN - M)           # exponent of the result's last significand bit
     tie = up = False
     if E >= q:
         mant = N << (E - q)
     else:
-        sh = q - E
-        mant, rem, half = N >> sh, N & ((1 << sh) - 1), 1 << (sh - 1)
-        tie = rem == half
-        up = rem > half or (tie and (mant & 1 == 1 or ties_away))
-        mant += up
+        mant, tie, up = round_shift(N, q - E, mode)
     if mant == 1 << (M + 1):
         mant >>= 1
         q += 1
+    if q + M > BIAS:                       # beyond the largest finite binade
+        if mode == "truncate":
+            return inf(fmt, sign) - 1, tie, up
+        return inf(fmt, sign), tie, up
     if mant < 1 << M:                      # subnormal (q == EMIN - M)
         return sign << (W - 1) | mant, tie, up
     return sign << (W - 1) | (q + M + BIAS) << M | (mant - (1 << M)), tie, up
 
 
-def fma(fmt, x, a, b, detail=False, ties_away=False):
-    """RN(x * a + b) on bits, exactly as IEEE 754 defines it."""
+def _infinite(fmt, sp, np_, sb, nb, factor_zero):
+    """x * a + b when x, a or b is infinite (np_ None: the product is), or NaNResult."""
+    if np_ is None and factor_zero:
+        raise NaNResult("0 * inf")
+    if np_ is None and nb is None and sp != sb:
+        raise NaNResult("inf - inf")
+    return inf(fmt, sp if np_ is None else sb)
+
+
+def fma(fmt, x, a, b, detail=False, ties_away=False, mode="rne"):
+    """RN(x * a + b) on bits, exactly as IEEE 754 defines it (round_rne's wrong rules on request)."""
     sx, nx, ex = decode(fmt, x)
     sa, na, ea = decode(fmt, a)
     sb, nb, eb = decode(fmt, b)
-    sp, np_, ep = sx ^ sa, nx * na, ex + ea
+    sp = sx ^ sa
+    if nx is None or na is None or nb is None:
+        np_ = None if nx is None or na is None else nx * na
+        r = (_infinite(fmt, sp, np_, sb, nb, nx == 0 or na == 0), False, False)
+        return r if detail else r[0]
+    np_, ep = nx * na, ex + ea
     e = min(ep, eb)
     v = (-1) ** sp * (np_ << (ep - e)) + (-1) ** sb * (nb << (eb - e))
     W = BIN[fmt][0]
@@ -119,7 +170,7 @@ def fma(fmt, x, a, b, detail=False, ties_away=False):
         zero_sign = (sp & sb) if (np_ == 0 and nb == 0) else 0
         r = (zero_sign << (W - 1), False, False)
     else:
-        r = round_rne(fmt, 1 if v < 0 else 0, abs(v), e, ties_away)
+        r = round_rne(fmt, 1 if v < 0 else 0, abs(v), e, ties_away, mode)
     return r if detail else r[0]
 
 
@@ -127,6 +178,8 @@ def mul(fmt, x, a):
     """RN(x * a)."""
     sx, nx, ex = decode(fmt, x)
     sa, na, ea = decode(fmt, a)
+    if nx is None or na is None:
+        return _infinite(fmt, sx ^ sa, None, 0, 0, nx == 0 or na == 0)
     if nx * na == 0:
         return (sx ^ sa) << (BIN[fmt][0] - 1)
     return round_rne(fmt, sx ^ sa, nx * na, ex + ea)[0]
@@ -186,8 +239,11 @@ def fma_thread(seed, fmt, tile, t):
             b[k] = mul(fmt, xv, pow2) ^ sbit
         elif name == "zero_neg":
             a[k], b[k] = ((xv >> (W - 1) & 1) ^ 1) << (W - 1), sbit
-        else:  # sticky
+        elif name == "sticky":
             a[k], b[k] = pow2, make(fmt, sb, q + M + 1, b[k] & ~1)
+        else:  # subnormal_operand: a subnormal with its top stored bit set, b normal in [2^EMIN, 2^(EMIN + 4))
+            a[k] = make(fmt, sa, EMIN - 1, a[k] | 1 << (M - 1))
+            b[k] = make(fmt, sb, uniform(draw(NX + NAB + k, 3), EMIN, EMIN + 3), b[k])
     return x, a, b
 
 
@@ -238,6 +294,12 @@ def classify(fmt, x, a, b):
     # b dominates: x * a lies wholly below b's last significand bit, and still moves the rounded result off b
     if p and (nb << (eb - e)) >= (p << (ex + ea - e)) << M and r != b:
         out.add("sticky")
+    # a multiplicand is subnormal, and reading it as a signed zero would change the result
+    for v, other, first in ((x, a, True), (a, x, False)):
+        if v & ((1 << (W - 1)) - 1) and exponent(fmt, v) == EMIN - 1:
+            z = v & (1 << (W - 1))
+            if fma(fmt, *((z, other) if first else (other, z)), b) != r:
+                out.add("subnormal_operand")
     return out
 
 

@@ -4,6 +4,7 @@
 // b2dp_fp_test against tests/fp_test_oracle.py:
 //   tile <seed> <fmt> <tile>   -> the operand table ([slot][thread] values' bits), then every thread's result words,
 //                                 then the kCtThreads check values
+//   fma <fmt> <x> <a> <b>      -> ft_fma on the operands' bits (std::fmaf / std::fma), the host's reference
 //   fold <n> <w0..wn-1>        -> ft_fold
 //   time <seed>                -> milliseconds to build every tile of every format (what one b2dp_fp_test call builds)
 //   bounds                     -> the constants the static_asserts bound
@@ -38,6 +39,11 @@ int main() {
             for (uint32_t w : t.words) std::printf(" %u", w);
             for (uint32_t c : t.check) std::printf(" %u", c);
             std::printf("\n");
+        } else if (op == "fma") {
+            int fmt;
+            unsigned long long x, a, b;
+            in >> fmt >> x >> a >> b;
+            std::printf("%llu\n", (unsigned long long)ft_fma(fmt, x, a, b));
         } else if (op == "fold") {
             int n;
             in >> n;
