@@ -270,8 +270,9 @@ typedef struct b2dp_probe_result {
                                       last b2dp_probe_reset) => Unhealthy, sticky */
 #define B2DP_RES_MEMTEST 0x200u    /* a b2dp_memtest of this device failed or timed out since open (or the last
                                       b2dp_probe_reset) => Unhealthy, sticky */
-#define B2DP_RES_COMPUTE 0x400u    /* a compute or FP self-test (b2dp_compute_test, b2dp_fp_test) of this device failed
-                                      or timed out since open (or the last b2dp_probe_reset) => Unhealthy, sticky */
+#define B2DP_RES_COMPUTE 0x400u    /* a compute, FP or SFU self-test (b2dp_compute_test, b2dp_fp_test, b2dp_sfu_test) of
+                                      this device failed or timed out since open (or the last b2dp_probe_reset) =>
+                                      Unhealthy, sticky */
 
 /* Replaces the exporter round trip getGPUHealth (exporter/health.go:42-82) and the evidence behind simpleHealthCheck
  * (plugin.go:161-206): launch the probe on every GPU of the context concurrently (one worker thread + stream per
@@ -283,7 +284,7 @@ B2DP_API int b2dp_probe_health(b2dp_ctx *ctx, const b2dp_probe_opts *opts, b2dp_
  * event numbered `mask` for `device` (seen by contexts opened with xid=1).  The reference has no equivalent. */
 B2DP_API int b2dp_probe_inject_fault(b2dp_ctx *ctx, int device, uint64_t word_index, uint32_t mask);
 /* Re-fill the probe buffers of `device` (-1 = all) with a clean pattern; also clears a latched Xid, a latched memtest
- * failure and a latched compute- or FP-test failure. */
+ * failure and a latched compute-, FP- or SFU-test failure. */
 B2DP_API int b2dp_probe_reset(b2dp_ctx *ctx, int device);
 /* Set the bandwidth ceiling (gbs_ref) of `device` (-1 = all) the fractional floor refers to, e.g. to the site's measured
  * HBM peak; gbs_ref <= 0 restores the device's own calibration.  Also how tests move a device across the 0.8 line. */
@@ -395,6 +396,8 @@ typedef struct b2dp_compute_test_result {
 #define B2DP_CT_SKIPPED_BUSY 0x1u      /* another process uses the GPU: nothing ran, nothing latched;
                                           healthy = the last heartbeat verdict */
 #define B2DP_CT_PARTIAL_COVERAGE 0x2u  /* sms_covered < sm_count: some SM ran no CTA of some format (reported, not failed) */
+#define B2DP_CT_NO_CONSENSUS 0x4u      /* b2dp_sfu_test: some result word had no strict majority over the SMs (Unhealthy) */
+#define B2DP_CT_OUT_OF_BOUND 0x8u      /* b2dp_sfu_test: some majority result failed the host's error bound (Unhealthy) */
 
 /* An on-demand check of the SMs' tensor cores on `device` (-1 = every GPU, concurrently on their workers): evidence
  * behind the per-GPU verdict the exporter round trip supplies in the reference (exporter/health.go:42-82), merged the
@@ -426,6 +429,30 @@ B2DP_API int b2dp_compute_test(b2dp_ctx *ctx, int device, const b2dp_compute_tes
  * B2DP_E_UNSUPPORTED otherwise. */
 B2DP_API int b2dp_fp_test(b2dp_ctx *ctx, int device, const b2dp_compute_test_opts *opts, b2dp_compute_test_result *out,
                           int cap, int *n);
+
+/* ---- on-demand SFU self-test (same opts, result and latch as the tensor-core self-test) ---- */
+#define B2DP_SF_F32 0              /* b2dp_sfu_test's format index: ex2, lg2, sin + cos, tanh (f32) */
+#define B2DP_SF_ROOT 1             /* rcp, rsqrt, sqrt (f32); rcp, rsqrt (f64) */
+#define B2DP_SF_F16 2              /* ex2, tanh (f16x2) */
+
+/* An on-demand check of the SMs' special-function units (MUFU: the .approx transcendentals) on `device` (-1 = every
+ * GPU, concurrently on their workers): evidence behind the per-GPU verdict the exporter round trip supplies in the
+ * reference (exporter/health.go:42-82), merged the same way (exporter/health.go:86-106) through the sticky
+ * B2DP_RES_COMPUTE bit.  NVIDIA publishes no bit-level model of MUFU, so the host cannot compute the results; per GPU
+ * and per format sfu_selftest.cuh first runs a reference launch of one CTA on every SM, the host takes each result
+ * word's strict majority over the SMs (B2DP_CT_NO_CONSENSUS where there is none), counts every CTA that differs from it
+ * in mismatches[] and bad_sm_mask, and checks every majority result against a loose bound of the exact function or its
+ * specials class (B2DP_CT_OUT_OF_BOUND).  A timed launch then fills every SM for duration_ms and compares every
+ * repetition with check values folded from the majority.  Operands: random values plus crafted exact points, domain
+ * edges, overflow, underflow, subnormal inputs, signed zeros, infinities, NaN and saturation.  The result struct is
+ * b2dp_compute_test_result with its per-format arrays indexed by B2DP_SF_*; tflops[] counts one op per MUFU result
+ * (T results/s).  Healthy iff the timed launches are healthy as b2dp_compute_test's, every reference record arrived,
+ * every word has a majority, no reference CTA dissents and every majority result passes the bound.  timeout_ms covers
+ * the reference launches and the timed launches together.  Latching, the probe lock, the busy skip and the release of
+ * every allocation are exactly b2dp_compute_test's.  cuda: backend with the in-process probe only; B2DP_E_UNSUPPORTED
+ * otherwise. */
+B2DP_API int b2dp_sfu_test(b2dp_ctx *ctx, int device, const b2dp_compute_test_opts *opts,
+                           b2dp_compute_test_result *out, int cap, int *n);
 
 /* exporter/health.go:86-106 PopulatePerGPUDHealth(devs, defaultHealth) merge rule.
  * have_source = 0 reproduces "exporter socket absent / RPC failed" (every device gets the

@@ -46,6 +46,8 @@ CT_EVEN_IF_BUSY = 1
 CT_SKIPPED_BUSY, CT_PARTIAL_COVERAGE = 1, 2
 CT_BF16, CT_FP8, CT_INT8 = 0, 1, 2
 FT_FP32, FT_FP64, FT_DMMA = 0, 1, 2
+SF_F32, SF_ROOT, SF_F16 = 0, 1, 2
+CT_NO_CONSENSUS, CT_OUT_OF_BOUND = 4, 8
 
 Id64 = C.c_char * 64
 
@@ -181,6 +183,7 @@ SIGNATURES = {
     "b2dp_memtest": (_i, [_vp, _i, _P(MemtestOpts), _P(MemtestResult), _i, _ip]),
     "b2dp_compute_test": (_i, [_vp, _i, _P(ComputeTestOpts), _P(ComputeTestResult), _i, _ip]),
     "b2dp_fp_test": (_i, [_vp, _i, _P(ComputeTestOpts), _P(ComputeTestResult), _i, _ip]),
+    "b2dp_sfu_test": (_i, [_vp, _i, _P(ComputeTestOpts), _P(ComputeTestResult), _i, _ip]),
     "b2dp_probe_set_ref": (_i, [_vp, _i, C.c_float]),
     "b2dp_probe_describe": (_i, [_vp, _i, _P(ProbeInfo)]),
     "b2dp_expected_checksum": (_i, [C.c_uint64, C.c_uint32, _P(C.c_uint64)]),

@@ -62,7 +62,8 @@ class ComputeTestResult:
     first_bad_format: int
     first_bad_tile: int
     ms: List[float]
-    tflops: List[float]            # 2 M N K x result tiles compared / ms (TOPS for INT8; fp_test: 2 x FMAs / ms)
+    tflops: List[float]            # 2 M N K x result tiles compared / ms (TOPS for INT8; fp_test: 2 x FMAs / ms;
+                                   # sfu_test: MUFU results / ms, in T results/s)
 
     def bad_sms(self) -> List[int]:
         return [s for s in range(256) if (self.bad_sm_mask[s // 64] >> (s % 64)) & 1]
@@ -235,6 +236,22 @@ class Context:
         opts = N.ComputeTestOpts(duration_ms, timeout_ms, N.CT_EVEN_IF_BUSY if even_if_busy else 0, fault_sm, fault_mask, 0)
         rc, arr, n = N.grow_call(lambda cap: (N.ComputeTestResult * cap)(),
                                  lambda a, cap, pn: N.lib.b2dp_fp_test(self._h, device, C.byref(opts), a, cap, pn))
+        N.check(rc, self._h)
+        return [ComputeTestResult(r.device, bool(r.healthy), r.err, r.flags, r.seed, r.sm_count, r.nsmid, r.sms_covered,
+                                  list(r.bad_sm_mask), list(r.mismatches), r.first_bad_sm, r.first_bad_format,
+                                  r.first_bad_tile, list(r.ms), list(r.tflops)) for r in arr[:n]]
+
+    def sfu_test(self, device: int = -1, duration_ms: int = 0, timeout_ms: int = 0, even_if_busy: bool = False,
+                 fault_sm: int = -1, fault_mask: int = 0) -> List[ComputeTestResult]:
+        """On-demand SFU self-test of `device` (-1 = every GPU, b2dp_sfu_test): a reference launch of one CTA per SM
+        whose result words' majority is bounded against the exact functions on the host, every dissenting SM named; then
+        the MUFU ops on every SM for duration_ms per format (0 = 1000), compared with the majority.  The per-format
+        lists are indexed by SF_F32, SF_ROOT, SF_F16; flags may carry CT_NO_CONSENSUS / CT_OUT_OF_BOUND.  A failure is
+        latched like compute_test()'s (RES_COMPUTE until probe_reset()); fault_sm / fault_mask flips bits of one result
+        on the SM with that %smid, in both launches."""
+        opts = N.ComputeTestOpts(duration_ms, timeout_ms, N.CT_EVEN_IF_BUSY if even_if_busy else 0, fault_sm, fault_mask, 0)
+        rc, arr, n = N.grow_call(lambda cap: (N.ComputeTestResult * cap)(),
+                                 lambda a, cap, pn: N.lib.b2dp_sfu_test(self._h, device, C.byref(opts), a, cap, pn))
         N.check(rc, self._h)
         return [ComputeTestResult(r.device, bool(r.healthy), r.err, r.flags, r.seed, r.sm_count, r.nsmid, r.sms_covered,
                                   list(r.bad_sm_mask), list(r.mismatches), r.first_bad_sm, r.first_bad_format,

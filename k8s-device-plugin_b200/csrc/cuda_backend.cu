@@ -36,6 +36,7 @@
 #include "nvml_dyn.hpp"
 #include "pattern_math.hpp"
 #include "fp_selftest.cuh"
+#include "sfu_selftest.cuh"
 #include "tc_selftest.cuh"
 #include "units_backend.hpp"
 
@@ -1571,12 +1572,16 @@ static int cuda_memtest(CudaBackend* be, int device, const b2dp_memtest_opts* op
     return B2DP_OK;
 }
 
-// ---- on-demand compute self-tests (b2dp_compute_test, b2dp_fp_test) -----------------------------------------------
-// One launch per format on one GPU, on that GPU's worker: tc_selftest.cuh (tensor cores: BF16, FP8, INT8) or
-// fp_selftest.cuh (FP32 FMA, FP64 FMA, FP64 tensor cores).  The host builds every operand table and every comparison
-// value itself (compute_test_math.hpp, fp_test_math.hpp): a health test must not ask the device under test for its own
-// reference values.  Both tests share this driver -- grid sizing, records, tally, deadline, busy skip and the release
-// of every allocation before the job ends, whatever happened -- through a DiagSuite.
+// ---- on-demand compute self-tests (b2dp_compute_test, b2dp_fp_test, b2dp_sfu_test) -----------------------------------
+// One launch per format on one GPU, on that GPU's worker: tc_selftest.cuh (tensor cores: BF16, FP8, INT8),
+// fp_selftest.cuh (FP32 FMA, FP64 FMA, FP64 tensor cores) or sfu_selftest.cuh (the special-function unit).  The host
+// builds every operand table and every comparison value itself (compute_test_math.hpp, fp_test_math.hpp): a health test
+// must not ask the device under test for its own reference values.  The SFU test departs from that rule, because no
+// bit-level model of MUFU is published: its reference step (sfu_reference) runs one CTA on every SM, takes each result
+// word's majority over the SMs, names every SM that disagrees, and bounds the majority against the exact function on
+// the host; no SM is ever judged against its own output.  The tests share this driver -- grid sizing, records, tally,
+// deadline, busy skip and the release of every allocation before the job ends, whatever happened -- through a
+// DiagSuite.
 constexpr uint32_t kComputeTestDefaultMs = 1000;
 
 using CtKernel = void (*)(const uint8_t*, const uint32_t*, unsigned long long, int, uint32_t, CtRecord*,
@@ -1586,6 +1591,14 @@ using CtKernel = void (*)(const uint8_t*, const uint32_t*, unsigned long long, i
 struct DiagTables {
     std::vector<uint8_t> tables[kCtFormats];
     std::vector<uint32_t> checks[kCtFormats];
+};
+
+// What a reference step found on one GPU.
+struct DiagRef {
+    bool run = true;    // every reference record arrived and every word has a majority: the timed launches can run
+    bool clean = true;  // and no CTA dissents from the majority, and every majority result passes the guard
+    int bad_sm[kCtFormats] = {-1, -1, -1};    // per format: the lowest dissenting SM id, and its CTA's first bad tile
+    int bad_tile[kCtFormats] = {-1, -1, -1};
 };
 
 struct DiagSuite {
@@ -1599,6 +1612,13 @@ struct DiagSuite {
     double (*macs_per_tile)(int fmt);          // multiply-adds of one comparison
     bool per_device_seed;                      // seed ^ (device << 16) per GPU, tables built on each worker; else one
                                                // seed and one set of tables per call
+    // Optional step on the worker before the timed launches (the SFU test's reference launch; null for the tensor and
+    // FP tests): fills `own` with this GPU's tables and checks, `ref` and r's reference tallies.
+    // Its deadline is the call's: the timed launches get what is left of timeout_ms.
+    cudaError_t (*reference)(Gpu* g, const b2dp_compute_test_opts& o, std::chrono::steady_clock::time_point deadline,
+                             const DiagTables& in, DiagTables& own, DiagRef& ref, b2dp_compute_test_result* r,
+                             const char** where, bool* timed_out);
+    const char* rate_format;                   // the log's tflops[] text; null: "%.0f/%.0f/%.0f TFLOP/s"
 };
 
 static void ct_suite_tile(uint32_t seed, int fmt, int tile, uint8_t* table, uint32_t* check) {
@@ -1626,6 +1646,105 @@ static const DiagSuite kTensorSuite = {"compute test", "tc_selftest", "bf16/fp8/
                                        ct_suite_tile, ct_macs_per_tile, true};
 static const DiagSuite kFpSuite = {"FP test", "fp_selftest", "fp32/fp64/dmma", kFtKernels, kFtSmem, kFtTableBytes,
                                    ft_suite_tile, ft_macs_per_tile, false};
+
+// ---- the SFU test's suite and reference step ----
+static_assert(kSfNoConsensus == B2DP_CT_NO_CONSENSUS && kSfOutOfBound == B2DP_CT_OUT_OF_BOUND, "sfu_test_math.hpp flags");
+constexpr int kSfRefSmem = 120 << 10;  // more than half an SM's shared memory, unused: no SM can hold two reference CTAs
+static const CtKernel kSfKernels[kSfFormats] = {sfu_selftest<SF_F32, false>, sfu_selftest<SF_ROOT, false>,
+                                                sfu_selftest<SF_F16, false>};
+static const CtKernel kSfRefKernels[kSfFormats] = {sfu_selftest<SF_F32, true>, sfu_selftest<SF_ROOT, true>,
+                                                   sfu_selftest<SF_F16, true>};
+static const uint32_t kSfSmem[kSfFormats] = {0, 0, 0};
+static const uint32_t kSfTableBytes[kSfFormats] = {sf_table_bytes(SF_F32), sf_table_bytes(SF_ROOT),
+                                                   sf_table_bytes(SF_F16)};
+// The operand tables only: the checks come from each GPU's reference launch.
+static void sf_suite_tile(uint32_t seed, int fmt, int tile, uint8_t* table, uint32_t* check) {
+    sf_build_table(seed, fmt, tile, reinterpret_cast<uint32_t*>(table));
+    memset(check, 0, kCtThreads * sizeof(uint32_t));
+}
+// tflops[] = 2 x this x comparisons / ms, and the SFU test counts one op per MUFU result
+static double sf_suite_half_results(int fmt) { return 0.5 * sf_results_per_tile(fmt); }
+
+// The reference launch of every format (kSfRefKernels: g->sms CTAs, one round, one per SM because of their shared
+// memory, every result word of round 0, repetition 0 dumped), then sf_consensus on each: this GPU's checks, its
+// dissenting SMs (counted in mismatches[] and bad_sm_mask), B2DP_CT_NO_CONSENSUS / B2DP_CT_OUT_OF_BOUND, and
+// B2DP_CT_PARTIAL_COVERAGE if the records name fewer SM ids than the device has.  Releases what it allocated.
+static cudaError_t sfu_reference(Gpu* g, const b2dp_compute_test_opts& o,
+                                 std::chrono::steady_clock::time_point deadline, const DiagTables& in, DiagTables& own,
+                                 DiagRef& ref, b2dp_compute_test_result* r, const char** where, bool* timed_out) {
+    const auto t0 = std::chrono::steady_clock::now();
+    const int n = (int)g->sms;
+    uint8_t* tab = nullptr;
+    uint32_t* dump = nullptr;
+    CtRecord* rec_h = nullptr;
+    CtRecord* rec_d = nullptr;
+    cudaEvent_t ev = nullptr;
+    cudaError_t ce = cudaSuccess;
+    std::vector<uint32_t> words((size_t)n * kCtTiles * kCtThreads * kSfMaxWords);
+    size_t table_max = 0;
+    for (int f = 0; f < kSfFormats; ++f) table_max = std::max(table_max, in.tables[f].size());
+#define SF_TRY(x) if ((ce = (x)) != cudaSuccess) { *where = #x; goto out; }
+    SF_TRY(cudaMalloc(&tab, table_max));
+    SF_TRY(cudaMalloc(&dump, words.size() * sizeof(uint32_t)));
+    SF_TRY(cudaHostAlloc(&rec_h, (size_t)kSfFormats * n * sizeof(CtRecord), cudaHostAllocMapped));
+    memset(rec_h, 0, (size_t)kSfFormats * n * sizeof(CtRecord));
+    SF_TRY(cudaHostGetDevicePointer(&rec_d, rec_h, 0));
+    SF_TRY(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+    for (int f = 0; f < kSfFormats; ++f) {
+        SF_TRY(cudaFuncSetAttribute(kSfRefKernels[f], cudaFuncAttributeMaxDynamicSharedMemorySize, kSfRefSmem));
+        SF_TRY(cudaFuncSetAttribute(kSfRefKernels[f], cudaFuncAttributePreferredSharedMemoryCarveout, 100));
+        SF_TRY(cudaMemcpy(tab, in.tables[f].data(), in.tables[f].size(), cudaMemcpyHostToDevice));
+        const unsigned long long seq = (unsigned long long)(f + 1);
+        kSfRefKernels[f]<<<n, kCtThreads, kSfRefSmem, g->stream>>>(tab, nullptr, 0ull, o.fault_sm, o.fault_mask,
+                                                                     rec_d + (size_t)f * n, seq, dump);
+        SF_TRY(cudaGetLastError());
+        SF_TRY(cudaEventRecord(ev, g->stream));
+        for (;;) {
+            const cudaError_t q = cudaEventQuery(ev);
+            if (q == cudaSuccess) break;
+            if (q != cudaErrorNotReady) { ce = q; *where = "sfu_selftest (reference launch)"; goto out; }
+            if (std::chrono::steady_clock::now() > deadline) { *timed_out = true; break; }
+            std::this_thread::sleep_for(std::chrono::milliseconds(1));
+        }
+        SF_TRY(cudaEventSynchronize(ev));  // the buffers can only be released once the kernel is done
+        if (*timed_out) goto out;
+        std::atomic_thread_fence(std::memory_order_acquire);
+        SF_TRY(cudaMemcpy(words.data(), dump, (size_t)n * kCtTiles * kCtThreads * kSfWords[f] * sizeof(uint32_t),
+                          cudaMemcpyDeviceToHost));
+        const CtRecord* recs = rec_h + (size_t)f * n;
+        SfConsensus cons;
+        sf_consensus(f, words.data(), recs, n, seq, reinterpret_cast<const uint32_t*>(in.tables[f].data()), cons);
+        own.tables[f] = in.tables[f];
+        own.checks[f] = cons.check;
+        for (int c = 0; c < n; ++c)
+            if (recs[c].seq == seq) r->nsmid = std::max<int32_t>(r->nsmid, (int32_t)recs[c].nsmid);
+        r->flags |= cons.flags();
+        if (cons.sm_ids < r->sm_count) r->flags |= B2DP_CT_PARTIAL_COVERAGE;
+        r->mismatches[f] += cons.dissents;
+        for (int i = 0; i < 4; ++i) r->bad_sm_mask[i] |= cons.bad_sm_mask[i];
+        ref.bad_sm[f] = cons.first_bad_sm;
+        ref.bad_tile[f] = cons.first_bad_tile;
+        if (cons.arrived != n || cons.no_consensus) ref.run = false;
+        if (!cons.clean()) ref.clean = false;
+        logf(cons.clean() ? 0 : 2, "%s SFU test reference %s: %d/%d records, %d SM ids, %llu dissents, %llu words "
+             "without a majority, %llu results out of bound", g->dev.id.c_str(), f == SF_F32 ? "f32" : f == SF_ROOT ? "root" : "f16",
+             cons.arrived, n, cons.sm_ids, cons.dissents, cons.no_consensus, cons.out_of_bound);
+    }
+    logf(0, "%s SFU test reference launches and consensus: %.1f ms", g->dev.id.c_str(),
+         std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count());
+out:
+#undef SF_TRY
+    if (g->stream) cudaStreamSynchronize(g->stream);
+    if (tab) cudaFree(tab);
+    if (dump) cudaFree(dump);
+    if (rec_h) cudaFreeHost(rec_h);
+    if (ev) cudaEventDestroy(ev);
+    return ce;
+}
+
+static const DiagSuite kSfuSuite = {"SFU test", "sfu_selftest", "f32/root/f16", kSfKernels, kSfSmem, kSfTableBytes,
+                                    sf_suite_tile, sf_suite_half_results, false, sfu_reference,
+                                    "%.2f/%.2f/%.2f T results/s"};
 
 static std::shared_ptr<DiagTables> diag_build_tables(const DiagSuite& su, uint32_t seed) {
     auto t = std::make_shared<DiagTables>();
@@ -1676,6 +1795,17 @@ static void compute_test_one(const DiagSuite& su, Gpu* g, const b2dp_compute_tes
         memset(rec_h, 0, (size_t)off[kCtFormats] * sizeof(CtRecord));
         CT_TRY(cudaHostGetDevicePointer(&rec_d, rec_h, 0));
         if (!tabs) tabs = diag_build_tables(su, r->seed);
+        DiagRef ref;
+        std::chrono::steady_clock::duration ref_spent{0};  // counts against the same timeout_ms as the timed launches
+        if (su.reference) {
+            auto own = std::make_shared<DiagTables>();
+            const auto t_ref = std::chrono::steady_clock::now();
+            ce = su.reference(g, o, t_ref + std::chrono::milliseconds(timeout_ms), *tabs, *own, ref, r, &where,
+                              &timed_out);
+            ref_spent = std::chrono::steady_clock::now() - t_ref;
+            if (ce != cudaSuccess || timed_out || !ref.run) goto done;  // Unhealthy; the timed launches do not run
+            tabs = own;
+        }
         for (int f = 0; f < kCtFormats; ++f) {
             const std::vector<uint8_t>& tables = tabs->tables[f];
             const std::vector<uint32_t>& checks = tabs->checks[f];
@@ -1694,7 +1824,7 @@ static void compute_test_one(const DiagSuite& su, Gpu* g, const b2dp_compute_tes
             CT_TRY(cudaGetLastError());
             CT_TRY(cudaEventRecord(ev[f + 1], g->stream));
         }
-        const auto deadline = std::chrono::steady_clock::now() + std::chrono::milliseconds(timeout_ms);
+        const auto deadline = std::chrono::steady_clock::now() + std::chrono::milliseconds(timeout_ms) - ref_spent;
         for (;;) {
             const cudaError_t q = cudaEventQuery(ev[kCtFormats]);
             if (q == cudaSuccess) break;
@@ -1729,6 +1859,10 @@ static void compute_test_one(const DiagSuite& su, Gpu* g, const b2dp_compute_tes
                     if (bad_sm < 0 || (int)c.smid < bad_sm) { bad_sm = (int)c.smid; bad_tile = c.first_bad_tile; }
                 }
             }
+            if (ref.bad_sm[f] >= 0 && (bad_sm < 0 || ref.bad_sm[f] < bad_sm)) {
+                bad_sm = ref.bad_sm[f];
+                bad_tile = ref.bad_tile[f];
+            }
             if (bad_sm >= 0 && r->first_bad_format < 0) {
                 r->first_bad_format = f;
                 r->first_bad_sm = bad_sm;
@@ -1738,7 +1872,7 @@ static void compute_test_one(const DiagSuite& su, Gpu* g, const b2dp_compute_tes
         }
         for (int s = 0; s < kCtMaxSmId; ++s) r->sms_covered += seen[0][s] && seen[1][s] && seen[2][s];
         if (r->sms_covered < r->sm_count) r->flags |= B2DP_CT_PARTIAL_COVERAGE;
-        r->healthy = compute_test_healthy(!timed_out, recs, seq) ? 1 : 0;
+        r->healthy = compute_test_healthy(!timed_out, recs, seq) && ref.clean ? 1 : 0;
     }
 done:
 #undef CT_TRY
@@ -1757,7 +1891,8 @@ done:
 static int cuda_diag_test(const DiagSuite& su, CudaBackend* be, int device, const b2dp_compute_test_opts* opts,
                           std::vector<b2dp_compute_test_result>& out, std::string& err) {
     if (be->units) {
-        err = std::string("the ") + (su.per_device_seed ? "compute self-test" : "FP self-test") +
+        err = std::string("the ") +
+              (su.per_device_seed ? "compute self-test" : su.reference ? "SFU self-test" : "FP self-test") +
               " runs in-process only (not with probe=helpers / probe=off / MIG)";
         return B2DP_E_UNSUPPORTED;
     }
@@ -1802,12 +1937,15 @@ static int cuda_diag_test(const DiagSuite& su, CudaBackend* be, int device, cons
             Gpu* g = be->gpus[sel[k]].get();
             const b2dp_compute_test_result& r = out[k];
             if (!r.healthy) { g->compute_fault.store(true); latched = true; }
+            char rate[96];
+            snprintf(rate, sizeof rate, su.rate_format ? su.rate_format : "%.0f/%.0f/%.0f TFLOP/s", r.tflops[0],
+                     r.tflops[1], r.tflops[2]);
             logf(r.healthy ? 0 : 2, "%s %s: %s, SMs %d/%d, mismatches %s %llu/%llu/%llu, first bad SM %d "
-                 "format %d tile %d, %.1f/%.1f/%.1f ms, %.0f/%.0f/%.0f TFLOP/s%s", g->dev.id.c_str(), su.log_name,
+                 "format %d tile %d, %.1f/%.1f/%.1f ms, %s%s", g->dev.id.c_str(), su.log_name,
                  r.healthy ? "Healthy" : "Unhealthy (latched)", r.sms_covered, r.sm_count, su.format_names,
                  (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
                  (unsigned long long)r.mismatches[2], r.first_bad_sm, r.first_bad_format, r.first_bad_tile, r.ms[0],
-                 r.ms[1], r.ms[2], r.tflops[0], r.tflops[1], r.tflops[2], r.err == B2DP_E_TIMEOUT ? ", timed out" : "");
+                 r.ms[1], r.ms[2], rate, r.err == B2DP_E_TIMEOUT ? ", timed out" : "");
         }
     }
     // like the Xid latch: running ListAndWatch loops send a heartbeat now (no backend lock is held while they do)
@@ -1825,6 +1963,11 @@ static int cuda_fp_test(CudaBackend* be, int device, const b2dp_compute_test_opt
     return cuda_diag_test(kFpSuite, be, device, opts, out, err);
 }
 
+static int cuda_sfu_test(CudaBackend* be, int device, const b2dp_compute_test_opts* opts,
+                         std::vector<b2dp_compute_test_result>& out, std::string& err) {
+    return cuda_diag_test(kSfuSuite, be, device, opts, out, err);
+}
+
 static bool cuda_diag_latched(CudaBackend* be) {
     for (auto& g : be->gpus)
         if (g->memtest_fault.load() || g->compute_fault.load()) return true;
@@ -1833,7 +1976,7 @@ static bool cuda_diag_latched(CudaBackend* be) {
 
 // registered when the library is loaded, before any entry point can run (internal.hpp DiagHooks)
 [[maybe_unused]] static const bool kDiagRegistered = [] {
-    diag_hooks() = DiagHooks{cuda_memtest, cuda_compute_test, cuda_fp_test, cuda_diag_latched};
+    diag_hooks() = DiagHooks{cuda_memtest, cuda_compute_test, cuda_fp_test, cuda_diag_latched, cuda_sfu_test};
     return true;
 }();
 

@@ -56,6 +56,8 @@ struct Flags {
     unsigned compute_test_ms = 0;                    // its duration per format (0 = 1000 ms)
     int fp_test_at_start = 0;                        // likewise for the FP32 / FP64 self-test (after the compute test);
                                                      // its duration per format is compute_test_ms too
+    int sfu_test_at_start = 0;                       // likewise for the SFU self-test (after the FP test), for
+                                                     // compute_test_ms per format
     bool version = false;
     bool labels_mode = false, reconcile = false, patch = false;
     std::string labels;                              // csv of generator names, or "all"
@@ -96,6 +98,7 @@ bool parse_flags(int argc, char** argv, Flags& f, std::string& err) {
         else if (name == "compute_test_at_start") f.compute_test_at_start = atoi(val.c_str());
         else if (name == "compute_test_ms") f.compute_test_ms = (unsigned)strtoul(val.c_str(), nullptr, 0);
         else if (name == "fp_test_at_start") f.fp_test_at_start = atoi(val.c_str());
+        else if (name == "sfu_test_at_start") f.sfu_test_at_start = atoi(val.c_str());
         else if (name == "labels") { f.labels_mode = true; f.labels = val; }
         else { err = "flag provided but not defined: -" + name; return false; }
     }
@@ -566,6 +569,32 @@ void run_fp_test(b2dp_ctx* ctx, const Flags& fl) {
     }
 }
 
+// -sfu_test_at_start=1: likewise for the SFU self-test (MUFU transcendentals, checked against the SMs' majority and
+// host error bounds), after the FP test, for -compute_test_ms per format.
+void run_sfu_test(b2dp_ctx* ctx, const Flags& fl) {
+    b2dp_compute_test_opts o{};
+    o.duration_ms = fl.compute_test_ms;
+    o.fault_sm = -1;
+    if (fl.sfu_test_at_start >= 2) o.flags |= B2DP_CT_EVEN_IF_BUSY;
+    b2dp_compute_test_result res[64];
+    int n = 0;
+    const int rc = b2dp_sfu_test(ctx, -1, &o, res, 64, &n);
+    if (rc != B2DP_OK) {
+        logf("sfu test at start not run: %s (%s)", b2dp_strerror(rc), b2dp_last_error(ctx));
+        return;
+    }
+    std::vector<b2dp_device> devs(n > 0 ? n : 1);
+    int nd = 0;
+    if (b2dp_enumerate(ctx, devs.data(), (int)devs.size(), &nd) != B2DP_OK) nd = 0;
+    for (int i = 0; i < n; ++i) {
+        const b2dp_compute_test_result& r = res[i];
+        logf("sfu test %s: %s, flags 0x%x, SMs %d/%d, mismatches %llu/%llu/%llu, first bad SM %d, %.2f/%.2f/%.2f "
+             "T results/s", r.device < nd ? devs[r.device].id : "?", r.healthy ? "Healthy" : "Unhealthy", r.flags,
+             r.sms_covered, r.sm_count, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
+             (unsigned long long)r.mismatches[2], r.first_bad_sm, r.tflops[0], r.tflops[1], r.tflops[2]);
+    }
+}
+
 }  // namespace
 
 int main(int argc, char** argv) {
@@ -599,6 +628,7 @@ int main(int argc, char** argv) {
     if (fl.memtest_at_start) run_memtest(ctx, fl);
     if (fl.compute_test_at_start) run_compute_test(ctx, fl);
     if (fl.fp_test_at_start) run_fp_test(ctx, fl);
+    if (fl.sfu_test_at_start) run_sfu_test(ctx, fl);
     char names[64][64];
     int n_res = 0;
     rc = b2dp_resource_list(ctx, fl.strategy.c_str(), names, 64, &n_res);  // main.go:141-146
