@@ -270,9 +270,9 @@ typedef struct b2dp_probe_result {
                                       last b2dp_probe_reset) => Unhealthy, sticky */
 #define B2DP_RES_MEMTEST 0x200u    /* a b2dp_memtest of this device failed or timed out since open (or the last
                                       b2dp_probe_reset) => Unhealthy, sticky */
-#define B2DP_RES_COMPUTE 0x400u    /* a compute, FP or SFU self-test (b2dp_compute_test, b2dp_fp_test, b2dp_sfu_test) of
-                                      this device failed or timed out since open (or the last b2dp_probe_reset) =>
-                                      Unhealthy, sticky */
+#define B2DP_RES_COMPUTE 0x400u    /* a compute, FP, SFU or shared-memory self-test (b2dp_compute_test, b2dp_fp_test,
+                                      b2dp_sfu_test, b2dp_smem_test) of this device failed or timed out since open (or
+                                      the last b2dp_probe_reset) => Unhealthy, sticky */
 
 /* Replaces the exporter round trip getGPUHealth (exporter/health.go:42-82) and the evidence behind simpleHealthCheck
  * (plugin.go:161-206): launch the probe on every GPU of the context concurrently (one worker thread + stream per
@@ -284,7 +284,7 @@ B2DP_API int b2dp_probe_health(b2dp_ctx *ctx, const b2dp_probe_opts *opts, b2dp_
  * event numbered `mask` for `device` (seen by contexts opened with xid=1).  The reference has no equivalent. */
 B2DP_API int b2dp_probe_inject_fault(b2dp_ctx *ctx, int device, uint64_t word_index, uint32_t mask);
 /* Re-fill the probe buffers of `device` (-1 = all) with a clean pattern; also clears a latched Xid, a latched memtest
- * failure and a latched compute-, FP- or SFU-test failure. */
+ * failure and a latched compute-, FP-, SFU- or shared-memory-test failure. */
 B2DP_API int b2dp_probe_reset(b2dp_ctx *ctx, int device);
 /* Set the bandwidth ceiling (gbs_ref) of `device` (-1 = all) the fractional floor refers to, e.g. to the site's measured
  * HBM peak; gbs_ref <= 0 restores the device's own calibration.  Also how tests move a device across the 0.8 line. */
@@ -398,6 +398,11 @@ typedef struct b2dp_compute_test_result {
 #define B2DP_CT_PARTIAL_COVERAGE 0x2u  /* sms_covered < sm_count: some SM ran no CTA of some format (reported, not failed) */
 #define B2DP_CT_NO_CONSENSUS 0x4u      /* b2dp_sfu_test: some result word had no strict majority over the SMs (Unhealthy) */
 #define B2DP_CT_OUT_OF_BOUND 0x8u      /* b2dp_sfu_test: some majority result failed the host's error bound (Unhealthy) */
+#define B2DP_CT_ECC_CORRECTED 0x10u    /* b2dp_smem_test: NVML's corrected ECC total grew during the launches (reported,
+                                          not failed) */
+#define B2DP_CT_ECC 0x20u              /* b2dp_smem_test: NVML's uncorrected ECC total grew during the launches
+                                          (Unhealthy) */
+#define B2DP_CT_NO_ECC 0x40u           /* b2dp_smem_test: NVML gave no ECC counters */
 
 /* An on-demand check of the SMs' tensor cores on `device` (-1 = every GPU, concurrently on their workers): evidence
  * behind the per-GPU verdict the exporter round trip supplies in the reference (exporter/health.go:42-82), merged the
@@ -453,6 +458,27 @@ B2DP_API int b2dp_fp_test(b2dp_ctx *ctx, int device, const b2dp_compute_test_opt
  * otherwise. */
 B2DP_API int b2dp_sfu_test(b2dp_ctx *ctx, int device, const b2dp_compute_test_opts *opts,
                            b2dp_compute_test_result *out, int cap, int *n);
+
+/* ---- on-demand shared-memory self-test (same opts, result and latch as the tensor-core self-test) ---- */
+#define B2DP_SH_WORD 0             /* b2dp_smem_test's format index: March C- with 32-bit accesses */
+#define B2DP_SH_BYTE 1             /* a march of 8-, 16-, 64- and 128-bit accesses (write enables, the wide data path) */
+#define B2DP_SH_DSMEM 2            /* clusters of two CTAs: every cell written and read by the peer SM (DSMEM) */
+
+/* An on-demand check of every SM's shared memory and of the SM-to-SM distributed-shared-memory path on `device` (-1 =
+ * every GPU, concurrently on their workers): evidence behind the per-GPU verdict the exporter round trip supplies in
+ * the reference (exporter/health.go:42-82), merged the same way (exporter/health.go:86-106) through the sticky
+ * B2DP_RES_COMPUTE bit.  smem_selftest.cuh runs one CTA of 227 KiB (the whole addressable array) on every SM and
+ * marches it under eight data backgrounds (solid, bit checkerboard, alternating bank rows, walking one, four keyed
+ * distinct-value tiles), writing every bit as 0 and as 1: March C- in 32-bit words (B2DP_SH_WORD), a mixed-width march
+ * (B2DP_SH_BYTE), and a march through the peer's window in clusters of two (B2DP_SH_DSMEM; a failure there names both
+ * SMs of the pair).  Every value read must equal the pattern, and every thread's fold of them the host's check value.
+ * tflops[] is TB/s of shared-memory traffic.  NVML's volatile ECC totals are read around the launches:
+ * B2DP_CT_ECC_CORRECTED (reported), B2DP_CT_ECC (Unhealthy), B2DP_CT_NO_ECC.  SH_DSMEM runs every co-resident cluster;
+ * if they do not cover every SM, B2DP_CT_PARTIAL_COVERAGE.  Verdict, latching, the probe lock, the busy skip and the
+ * release of every allocation are exactly b2dp_compute_test's.  cuda: backend with the in-process probe only;
+ * B2DP_E_UNSUPPORTED otherwise. */
+B2DP_API int b2dp_smem_test(b2dp_ctx *ctx, int device, const b2dp_compute_test_opts *opts,
+                            b2dp_compute_test_result *out, int cap, int *n);
 
 /* exporter/health.go:86-106 PopulatePerGPUDHealth(devs, defaultHealth) merge rule.
  * have_source = 0 reproduces "exporter socket absent / RPC failed" (every device gets the

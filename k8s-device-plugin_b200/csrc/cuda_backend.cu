@@ -37,6 +37,7 @@
 #include "pattern_math.hpp"
 #include "fp_selftest.cuh"
 #include "sfu_selftest.cuh"
+#include "smem_selftest.cuh"
 #include "tc_selftest.cuh"
 #include "units_backend.hpp"
 
@@ -1572,10 +1573,11 @@ static int cuda_memtest(CudaBackend* be, int device, const b2dp_memtest_opts* op
     return B2DP_OK;
 }
 
-// ---- on-demand compute self-tests (b2dp_compute_test, b2dp_fp_test, b2dp_sfu_test) -----------------------------------
+// ---- on-demand compute self-tests (b2dp_compute_test, b2dp_fp_test, b2dp_sfu_test, b2dp_smem_test) ------------------
 // One launch per format on one GPU, on that GPU's worker: tc_selftest.cuh (tensor cores: BF16, FP8, INT8),
-// fp_selftest.cuh (FP32 FMA, FP64 FMA, FP64 tensor cores) or sfu_selftest.cuh (the special-function unit).  The host
-// builds every operand table and every comparison value itself (compute_test_math.hpp, fp_test_math.hpp): a health test
+// fp_selftest.cuh (FP32 FMA, FP64 FMA, FP64 tensor cores), sfu_selftest.cuh (the special-function unit) or
+// smem_selftest.cuh (shared memory and the SM-to-SM DSMEM path).  The host builds every operand table and every
+// comparison value itself (compute_test_math.hpp, fp_test_math.hpp, smem_test_math.hpp): a health test
 // must not ask the device under test for its own reference values.  The SFU test departs from that rule, because no
 // bit-level model of MUFU is published: its reference step (sfu_reference) runs one CTA on every SM, takes each result
 // word's majority over the SMs, names every SM that disagrees, and bounds the majority against the exact function on
@@ -1619,6 +1621,11 @@ struct DiagSuite {
                              const DiagTables& in, DiagTables& own, DiagRef& ref, b2dp_compute_test_result* r,
                              const char** where, bool* timed_out);
     const char* rate_format;                   // the log's tflops[] text; null: "%.0f/%.0f/%.0f TFLOP/s"
+    // Optional grid sizing (the shared-memory test; null: every CTA of cudaOccupancyMaxActiveBlocksPerMultiprocessor
+    // on every SM), after the kernel's shared-memory attributes are set.  On an error it names the cause in *where.
+    cudaError_t (*size_grid)(Gpu* g, int fmt, int* grid, const char** where);
+    bool ecc;                                  // read NVML's volatile ECC totals around the timed launches
+    const char* test_name;                     // in the error of a backend without the test; null: by the fields above
 };
 
 static void ct_suite_tile(uint32_t seed, int fmt, int tile, uint8_t* table, uint32_t* check) {
@@ -1746,6 +1753,47 @@ static const DiagSuite kSfuSuite = {"SFU test", "sfu_selftest", "f32/root/f16", 
                                     sf_suite_tile, sf_suite_half_results, false, sfu_reference,
                                     "%.2f/%.2f/%.2f T results/s"};
 
+// ---- the shared-memory test's suite ----
+static const CtKernel kShKernels[kShFormats] = {smem_selftest<SH_WORD, false>, smem_selftest<SH_BYTE, false>,
+                                                smem_selftest<SH_DSMEM, false>};
+static const uint32_t kShSmem[kShFormats] = {kShBytes, kShBytes, kShBytes};
+static const uint32_t kShTableBytes[kShFormats] = {kShTableWords * 4, kShTableWords * 4, kShTableWords * 4};
+static void sh_suite_tile(uint32_t seed, int fmt, int tile, uint8_t* table, uint32_t* check) {
+    sh_build_tile(seed, fmt, tile, reinterpret_cast<uint32_t*>(table), check);
+}
+// tflops[] = 2 x this x comparisons / ms: TB/s of shared-memory traffic
+static double sh_suite_half_bytes(int fmt) { return 0.5 * sh_bytes_per_tile(fmt); }
+
+// One CTA per SM for SH_WORD / SH_BYTE (kShBytes each: no SM holds two); SH_DSMEM: every co-resident cluster of two.
+static cudaError_t sh_size_grid(Gpu* g, int fmt, int* grid, const char** where) {
+    int dev = 0, optin = 0;
+    cudaError_t ce = cudaGetDevice(&dev);
+    if (ce == cudaSuccess) ce = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+    if (ce != cudaSuccess) { *where = "cudaDeviceGetAttribute(cudaDevAttrMaxSharedMemoryPerBlockOptin)"; return ce; }
+    if (optin < (int)kShBytes) {
+        *where = "smem_selftest: the device's cudaDevAttrMaxSharedMemoryPerBlockOptin is below the 232448 B the test needs";
+        return cudaErrorInvalidConfiguration;
+    }
+    if (fmt != SH_DSMEM) { *grid = (int)g->sms; return cudaSuccess; }
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(2);
+    cfg.blockDim = dim3(kCtThreads);
+    cfg.dynamicSmemBytes = kShBytes;
+    int clusters = 0;
+    if ((ce = cudaOccupancyMaxActiveClusters(&clusters, kShKernels[SH_DSMEM], &cfg)) != cudaSuccess) {
+        *where = "cudaOccupancyMaxActiveClusters(smem_selftest<SH_DSMEM>)";
+        return ce;
+    }
+    if (clusters < 1) { *where = "smem_selftest<SH_DSMEM>: no cluster of two fits"; return cudaErrorInvalidConfiguration; }
+    logf(0, "%s shared-memory test: %d clusters of two CTAs co-resident (%u SMs)", g->dev.id.c_str(), clusters, g->sms);
+    *grid = 2 * clusters;
+    return cudaSuccess;
+}
+
+static const DiagSuite kSmemSuite = {"shared-memory test", "smem_selftest", "word/byte/dsmem", kShKernels, kShSmem,
+                                     kShTableBytes, sh_suite_tile, sh_suite_half_bytes, false, nullptr,
+                                     "%.2f/%.2f/%.2f TB/s", sh_size_grid, true, "shared-memory self-test"};
+
 static std::shared_ptr<DiagTables> diag_build_tables(const DiagSuite& su, uint32_t seed) {
     auto t = std::make_shared<DiagTables>();
     for (int f = 0; f < kCtFormats; ++f) {
@@ -1758,7 +1806,8 @@ static std::shared_ptr<DiagTables> diag_build_tables(const DiagSuite& su, uint32
     return t;
 }
 
-static void compute_test_one(const DiagSuite& su, Gpu* g, const b2dp_compute_test_opts& o, uint32_t duration_ms,
+static void compute_test_one(const DiagSuite& su, CudaBackend* be, Gpu* g, const b2dp_compute_test_opts& o,
+                             uint32_t duration_ms,
                              uint32_t timeout_ms, std::shared_ptr<const DiagTables> tabs, b2dp_compute_test_result* r,
                              std::string* err) {
     uint8_t* img[kCtFormats] = {};
@@ -1786,9 +1835,13 @@ static void compute_test_one(const DiagSuite& su, Gpu* g, const b2dp_compute_tes
         for (int f = 0; f < kCtFormats; ++f) {
             CT_TRY(cudaFuncSetAttribute(su.kernels[f], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)su.smem[f]));
             CT_TRY(cudaFuncSetAttribute(su.kernels[f], cudaFuncAttributePreferredSharedMemoryCarveout, 100));
-            int per_sm = 0;
-            CT_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, su.kernels[f], kCtThreads, su.smem[f]));
-            grid[f] = (int)g->sms * (per_sm > 0 ? per_sm : 1);  // every CTA resident at once
+            if (su.size_grid) {
+                if ((ce = su.size_grid(g, f, &grid[f], &where)) != cudaSuccess) goto done;
+            } else {
+                int per_sm = 0;
+                CT_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, su.kernels[f], kCtThreads, su.smem[f]));
+                grid[f] = (int)g->sms * (per_sm > 0 ? per_sm : 1);  // every CTA resident at once
+            }
             off[f + 1] = off[f] + grid[f];
         }
         CT_TRY(cudaHostAlloc(&rec_h, (size_t)off[kCtFormats] * sizeof(CtRecord), cudaHostAllocMapped));
@@ -1815,6 +1868,12 @@ static void compute_test_one(const DiagSuite& su, Gpu* g, const b2dp_compute_tes
             CT_TRY(cudaMemcpy(chk[f], checks.data(), checks.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
         }
         for (cudaEvent_t& e : ev) CT_TRY(cudaEventCreate(&e));
+        // Device-wide counters, as the memory test reads them: a single-bit defect ECC corrects never reaches the data
+        // check, and only the corrected count shows it.
+        unsigned long long corr0 = 0, unc0 = 0;
+        const bool ecc = su.ecc && g->nvh && be->nvml.ecc_total && be->nvml.ecc_total(g->nvh, 1, 0, &unc0) == 0 &&
+                         be->nvml.ecc_total(g->nvh, 0, 0, &corr0) == 0;
+        if (su.ecc && !ecc) r->flags |= B2DP_CT_NO_ECC;
 
         CT_TRY(cudaEventRecord(ev[0], g->stream));
         for (int f = 0; f < kCtFormats; ++f) {
@@ -1835,6 +1894,16 @@ static void compute_test_one(const DiagSuite& su, Gpu* g, const b2dp_compute_tes
         // past the deadline the verdict is made, but the buffers can only be released once the kernels are done
         CT_TRY(cudaEventSynchronize(ev[kCtFormats]));
         std::atomic_thread_fence(std::memory_order_acquire);
+        bool ecc_clean = true;
+        if (ecc) {
+            unsigned long long corr1 = corr0, unc1 = unc0;
+            be->nvml.ecc_total(g->nvh, 1, 0, &unc1);
+            be->nvml.ecc_total(g->nvh, 0, 0, &corr1);
+            if (corr1 > corr0) r->flags |= B2DP_CT_ECC_CORRECTED;
+            if (unc1 > unc0) { r->flags |= B2DP_CT_ECC; ecc_clean = false; }
+            logf(unc1 > unc0 ? 2 : 0, "%s %s: ECC totals corrected +%llu, uncorrected +%llu", g->dev.id.c_str(),
+                 su.log_name, corr1 - corr0, unc1 > unc0 ? unc1 - unc0 : 0ull);
+        }
 
         std::vector<CtRecord> recs[kCtFormats];
         unsigned long long seq[kCtFormats];
@@ -1872,7 +1941,7 @@ static void compute_test_one(const DiagSuite& su, Gpu* g, const b2dp_compute_tes
         }
         for (int s = 0; s < kCtMaxSmId; ++s) r->sms_covered += seen[0][s] && seen[1][s] && seen[2][s];
         if (r->sms_covered < r->sm_count) r->flags |= B2DP_CT_PARTIAL_COVERAGE;
-        r->healthy = compute_test_healthy(!timed_out, recs, seq) && ref.clean ? 1 : 0;
+        r->healthy = compute_test_healthy(!timed_out, recs, seq) && ref.clean && ecc_clean ? 1 : 0;
     }
 done:
 #undef CT_TRY
@@ -1892,7 +1961,10 @@ static int cuda_diag_test(const DiagSuite& su, CudaBackend* be, int device, cons
                           std::vector<b2dp_compute_test_result>& out, std::string& err) {
     if (be->units) {
         err = std::string("the ") +
-              (su.per_device_seed ? "compute self-test" : su.reference ? "SFU self-test" : "FP self-test") +
+              (su.test_name         ? su.test_name
+               : su.per_device_seed ? "compute self-test"
+               : su.reference       ? "SFU self-test"
+                                    : "FP self-test") +
               " runs in-process only (not with probe=helpers / probe=off / MIG)";
         return B2DP_E_UNSUPPORTED;
     }
@@ -1926,8 +1998,8 @@ static int cuda_diag_test(const DiagSuite& su, CudaBackend* be, int device, cons
             }
             std::string* e = &errs[k];
             const DiagSuite* sp = &su;
-            cs[k] = post(g, [sp, g, o, duration_ms, timeout_ms, shared, r, e] {
-                compute_test_one(*sp, g, o, duration_ms, timeout_ms, shared, r, e);
+            cs[k] = post(g, [sp, be, g, o, duration_ms, timeout_ms, shared, r, e] {
+                compute_test_one(*sp, be, g, o, duration_ms, timeout_ms, shared, r, e);
             });
         }
         for (size_t k = 0; k < sel.size(); ++k) {
@@ -1968,6 +2040,11 @@ static int cuda_sfu_test(CudaBackend* be, int device, const b2dp_compute_test_op
     return cuda_diag_test(kSfuSuite, be, device, opts, out, err);
 }
 
+static int cuda_smem_test(CudaBackend* be, int device, const b2dp_compute_test_opts* opts,
+                          std::vector<b2dp_compute_test_result>& out, std::string& err) {
+    return cuda_diag_test(kSmemSuite, be, device, opts, out, err);
+}
+
 static bool cuda_diag_latched(CudaBackend* be) {
     for (auto& g : be->gpus)
         if (g->memtest_fault.load() || g->compute_fault.load()) return true;
@@ -1976,7 +2053,8 @@ static bool cuda_diag_latched(CudaBackend* be) {
 
 // registered when the library is loaded, before any entry point can run (internal.hpp DiagHooks)
 [[maybe_unused]] static const bool kDiagRegistered = [] {
-    diag_hooks() = DiagHooks{cuda_memtest, cuda_compute_test, cuda_fp_test, cuda_diag_latched, cuda_sfu_test};
+    diag_hooks() = DiagHooks{cuda_memtest, cuda_compute_test, cuda_fp_test, cuda_diag_latched, cuda_sfu_test,
+                             cuda_smem_test};
     return true;
 }();
 
