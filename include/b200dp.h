@@ -270,9 +270,10 @@ typedef struct b2dp_probe_result {
                                       last b2dp_probe_reset) => Unhealthy, sticky */
 #define B2DP_RES_MEMTEST 0x200u    /* a b2dp_memtest of this device failed or timed out since open (or the last
                                       b2dp_probe_reset) => Unhealthy, sticky */
-#define B2DP_RES_COMPUTE 0x400u    /* a compute, FP, SFU or shared-memory self-test (b2dp_compute_test, b2dp_fp_test,
-                                      b2dp_sfu_test, b2dp_smem_test) of this device failed or timed out since open (or
-                                      the last b2dp_probe_reset) => Unhealthy, sticky */
+#define B2DP_RES_COMPUTE 0x400u    /* a compute, FP, SFU, shared-memory or register-file self-test (b2dp_compute_test,
+                                      b2dp_fp_test, b2dp_sfu_test, b2dp_smem_test, b2dp_regfile_test) of this device
+                                      failed or timed out since open (or the last b2dp_probe_reset) => Unhealthy,
+                                      sticky */
 
 /* Replaces the exporter round trip getGPUHealth (exporter/health.go:42-82) and the evidence behind simpleHealthCheck
  * (plugin.go:161-206): launch the probe on every GPU of the context concurrently (one worker thread + stream per
@@ -284,7 +285,7 @@ B2DP_API int b2dp_probe_health(b2dp_ctx *ctx, const b2dp_probe_opts *opts, b2dp_
  * event numbered `mask` for `device` (seen by contexts opened with xid=1).  The reference has no equivalent. */
 B2DP_API int b2dp_probe_inject_fault(b2dp_ctx *ctx, int device, uint64_t word_index, uint32_t mask);
 /* Re-fill the probe buffers of `device` (-1 = all) with a clean pattern; also clears a latched Xid, a latched memtest
- * failure and a latched compute-, FP-, SFU- or shared-memory-test failure. */
+ * failure and a latched compute-, FP-, SFU-, shared-memory- or register-file-test failure. */
 B2DP_API int b2dp_probe_reset(b2dp_ctx *ctx, int device);
 /* Set the bandwidth ceiling (gbs_ref) of `device` (-1 = all) the fractional floor refers to, e.g. to the site's measured
  * HBM peak; gbs_ref <= 0 restores the device's own calibration.  Also how tests move a device across the 0.8 line. */
@@ -479,6 +480,26 @@ B2DP_API int b2dp_sfu_test(b2dp_ctx *ctx, int device, const b2dp_compute_test_op
  * B2DP_E_UNSUPPORTED otherwise. */
 B2DP_API int b2dp_smem_test(b2dp_ctx *ctx, int device, const b2dp_compute_test_opts *opts,
                             b2dp_compute_test_result *out, int cap, int *n);
+
+/* ---- on-demand register-file self-test (same opts, result and latch as the tensor-core self-test) ---- */
+#define B2DP_RF_ALU 0              /* b2dp_regfile_test's format index: March C- by in-place ALU writes (LOP3) */
+#define B2DP_RF_LOAD 1             /* every held register written by 128- and 64-bit shared-memory loads */
+#define B2DP_RF_HOLD 2             /* P and ~P each held 100 us while the warps sleep (not a retention test) */
+
+/* An on-demand check of every SM's register file on `device` (-1 = every GPU, concurrently on their workers): evidence
+ * behind the per-GPU verdict the exporter round trip supplies in the reference (exporter/health.go:42-82), merged the
+ * same way (exporter/health.go:86-106) through the sticky B2DP_RES_COMPUTE bit.  rf_selftest.cuh runs two CTAs of 128
+ * threads on every SM (255 registers per thread, allocated as 256: the SM's whole 64 K-register file), and every
+ * thread holds 204 values in general registers across every step of a march under eight data backgrounds (solid, bit
+ * checkerboard, alternating registers, walking one, four keyed distinct-value tiles), writing every bit as 0 and as 1:
+ * March C- by in-place ALU writes (B2DP_RF_ALU), by wide shared-memory loads (B2DP_RF_LOAD), and P and ~P each held
+ * for 100 us while the warps sleep (B2DP_RF_HOLD).  Every value read must equal the pattern, and every thread's fold
+ * of them the host's check value.  tflops[] is TB/s of register data read and written.  NVML's volatile ECC totals are
+ * read around the launches: B2DP_CT_ECC_CORRECTED (reported), B2DP_CT_ECC (Unhealthy), B2DP_CT_NO_ECC.  Verdict,
+ * latching, the probe lock, the busy skip and the release of every allocation are exactly b2dp_compute_test's.  cuda:
+ * backend with the in-process probe only; B2DP_E_UNSUPPORTED otherwise. */
+B2DP_API int b2dp_regfile_test(b2dp_ctx *ctx, int device, const b2dp_compute_test_opts *opts,
+                               b2dp_compute_test_result *out, int cap, int *n);
 
 /* exporter/health.go:86-106 PopulatePerGPUDHealth(devs, defaultHealth) merge rule.
  * have_source = 0 reproduces "exporter socket absent / RPC failed" (every device gets the

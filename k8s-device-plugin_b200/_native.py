@@ -49,6 +49,7 @@ FT_FP32, FT_FP64, FT_DMMA = 0, 1, 2
 SF_F32, SF_ROOT, SF_F16 = 0, 1, 2
 CT_NO_CONSENSUS, CT_OUT_OF_BOUND = 4, 8
 SH_WORD, SH_BYTE, SH_DSMEM = 0, 1, 2
+RF_ALU, RF_LOAD, RF_HOLD = 0, 1, 2
 CT_ECC_CORRECTED, CT_ECC, CT_NO_ECC = 0x10, 0x20, 0x40
 
 Id64 = C.c_char * 64
@@ -187,6 +188,7 @@ SIGNATURES = {
     "b2dp_fp_test": (_i, [_vp, _i, _P(ComputeTestOpts), _P(ComputeTestResult), _i, _ip]),
     "b2dp_sfu_test": (_i, [_vp, _i, _P(ComputeTestOpts), _P(ComputeTestResult), _i, _ip]),
     "b2dp_smem_test": (_i, [_vp, _i, _P(ComputeTestOpts), _P(ComputeTestResult), _i, _ip]),
+    "b2dp_regfile_test": (_i, [_vp, _i, _P(ComputeTestOpts), _P(ComputeTestResult), _i, _ip]),
     "b2dp_probe_set_ref": (_i, [_vp, _i, C.c_float]),
     "b2dp_probe_describe": (_i, [_vp, _i, _P(ProbeInfo)]),
     "b2dp_expected_checksum": (_i, [C.c_uint64, C.c_uint32, _P(C.c_uint64)]),

@@ -36,6 +36,7 @@
 #include "nvml_dyn.hpp"
 #include "pattern_math.hpp"
 #include "fp_selftest.cuh"
+#include "rf_selftest.cuh"
 #include "sfu_selftest.cuh"
 #include "smem_selftest.cuh"
 #include "tc_selftest.cuh"
@@ -1573,12 +1574,13 @@ static int cuda_memtest(CudaBackend* be, int device, const b2dp_memtest_opts* op
     return B2DP_OK;
 }
 
-// ---- on-demand compute self-tests (b2dp_compute_test, b2dp_fp_test, b2dp_sfu_test, b2dp_smem_test) ------------------
+// ---- on-demand compute self-tests (b2dp_compute_test, b2dp_fp_test, b2dp_sfu_test, b2dp_smem_test,
+// b2dp_regfile_test) ---------------------------------------------------------------------------------------------------
 // One launch per format on one GPU, on that GPU's worker: tc_selftest.cuh (tensor cores: BF16, FP8, INT8),
-// fp_selftest.cuh (FP32 FMA, FP64 FMA, FP64 tensor cores), sfu_selftest.cuh (the special-function unit) or
-// smem_selftest.cuh (shared memory and the SM-to-SM DSMEM path).  The host builds every operand table and every
-// comparison value itself (compute_test_math.hpp, fp_test_math.hpp, smem_test_math.hpp): a health test
-// must not ask the device under test for its own reference values.  The SFU test departs from that rule, because no
+// fp_selftest.cuh (FP32 FMA, FP64 FMA, FP64 tensor cores), sfu_selftest.cuh (the special-function unit),
+// smem_selftest.cuh (shared memory and the SM-to-SM DSMEM path) or rf_selftest.cuh (the register file).  The host builds
+// every operand table and every comparison value itself (compute_test_math.hpp, fp_test_math.hpp, smem_test_math.hpp,
+// rf_test_math.hpp): a health test must not ask the device under test for its own reference values.  The SFU test departs from that rule, because no
 // bit-level model of MUFU is published: its reference step (sfu_reference) runs one CTA on every SM, takes each result
 // word's majority over the SMs, names every SM that disagrees, and bounds the majority against the exact function on
 // the host; no SM is ever judged against its own output.  The tests share this driver -- grid sizing, records, tally,
@@ -1793,6 +1795,23 @@ static cudaError_t sh_size_grid(Gpu* g, int fmt, int* grid, const char** where) 
 static const DiagSuite kSmemSuite = {"shared-memory test", "smem_selftest", "word/byte/dsmem", kShKernels, kShSmem,
                                      kShTableBytes, sh_suite_tile, sh_suite_half_bytes, false, nullptr,
                                      "%.2f/%.2f/%.2f TB/s", sh_size_grid, true, "shared-memory self-test"};
+
+// ---- the register-file test's suite ----
+// __launch_bounds__(kCtThreads, 2) and kRfSmemBytes each: the default grid sizing gives two CTAs on every SM, which
+// between them take the whole register file.
+static const CtKernel kRfKernels[kRfFormats] = {rf_selftest<RF_ALU, false>, rf_selftest<RF_LOAD, false>,
+                                                rf_selftest<RF_HOLD, false>};
+static const uint32_t kRfSmem[kRfFormats] = {kRfSmemBytes, kRfSmemBytes, kRfSmemBytes};
+static const uint32_t kRfTableBytes[kRfFormats] = {kRfTableWords * 4, kRfTableWords * 4, kRfTableWords * 4};
+static void rf_suite_tile(uint32_t seed, int fmt, int tile, uint8_t* table, uint32_t* check) {
+    rf_build_tile(seed, fmt, tile, reinterpret_cast<uint32_t*>(table), check);
+}
+// tflops[] = 2 x this x comparisons / ms: TB/s of register data the march reads and writes
+static double rf_suite_half_bytes(int fmt) { return 0.5 * rf_bytes_per_tile(fmt); }
+
+static const DiagSuite kRfSuite = {"register-file test", "rf_selftest", "alu/load/hold", kRfKernels, kRfSmem,
+                                   kRfTableBytes, rf_suite_tile, rf_suite_half_bytes, false, nullptr,
+                                   "%.2f/%.2f/%.2f TB/s", nullptr, true, "register-file self-test"};
 
 static std::shared_ptr<DiagTables> diag_build_tables(const DiagSuite& su, uint32_t seed) {
     auto t = std::make_shared<DiagTables>();
@@ -2045,6 +2064,11 @@ static int cuda_smem_test(CudaBackend* be, int device, const b2dp_compute_test_o
     return cuda_diag_test(kSmemSuite, be, device, opts, out, err);
 }
 
+static int cuda_regfile_test(CudaBackend* be, int device, const b2dp_compute_test_opts* opts,
+                             std::vector<b2dp_compute_test_result>& out, std::string& err) {
+    return cuda_diag_test(kRfSuite, be, device, opts, out, err);
+}
+
 static bool cuda_diag_latched(CudaBackend* be) {
     for (auto& g : be->gpus)
         if (g->memtest_fault.load() || g->compute_fault.load()) return true;
@@ -2054,7 +2078,7 @@ static bool cuda_diag_latched(CudaBackend* be) {
 // registered when the library is loaded, before any entry point can run (internal.hpp DiagHooks)
 [[maybe_unused]] static const bool kDiagRegistered = [] {
     diag_hooks() = DiagHooks{cuda_memtest, cuda_compute_test, cuda_fp_test, cuda_diag_latched, cuda_sfu_test,
-                             cuda_smem_test};
+                             cuda_smem_test, cuda_regfile_test};
     return true;
 }();
 

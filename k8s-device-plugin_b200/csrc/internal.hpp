@@ -146,7 +146,7 @@ void cuda_set_health_event_callback(CudaBackend*, std::function<void()> fn);
 // The on-demand diagnostics (the memory test and the compute and FP self-tests) are optional capabilities of the cuda backend:
 // a build of the library whose backend has none (the CPU-only build of ctx.cpp the sanitizer tests link against a
 // stand-in backend) simply leaves these null, and b2dp_memtest / b2dp_compute_test / b2dp_fp_test / b2dp_sfu_test /
-// b2dp_smem_test then return B2DP_E_UNSUPPORTED.
+// b2dp_smem_test / b2dp_regfile_test then return B2DP_E_UNSUPPORTED.
 // cuda_backend.cu fills them in during static initialisation.
 struct DiagHooks {
     // b2dp_memtest on `device` (-1 = all); B2DP_E_UNSUPPORTED without the in-process probe
@@ -158,8 +158,8 @@ struct DiagHooks {
     // b2dp_fp_test on `device` (-1 = all); B2DP_E_UNSUPPORTED without the in-process probe
     int (*fp_test)(CudaBackend*, int device, const b2dp_compute_test_opts* opts,
                    std::vector<b2dp_compute_test_result>& out, std::string& err) = nullptr;
-    // true while any device carries a latched memtest, compute-test, FP-test, SFU-test or shared-memory-test failure
-    // (cleared by b2dp_probe_reset)
+    // true while any device carries a latched memtest, compute-test, FP-test, SFU-test, shared-memory-test or
+    // register-file-test failure (cleared by b2dp_probe_reset)
     bool (*latched)(CudaBackend*) = nullptr;
     // b2dp_sfu_test on `device` (-1 = all); B2DP_E_UNSUPPORTED without the in-process probe
     int (*sfu_test)(CudaBackend*, int device, const b2dp_compute_test_opts* opts,
@@ -167,6 +167,9 @@ struct DiagHooks {
     // b2dp_smem_test on `device` (-1 = all); B2DP_E_UNSUPPORTED without the in-process probe
     int (*smem_test)(CudaBackend*, int device, const b2dp_compute_test_opts* opts,
                      std::vector<b2dp_compute_test_result>& out, std::string& err) = nullptr;
+    // b2dp_regfile_test on `device` (-1 = all); B2DP_E_UNSUPPORTED without the in-process probe
+    int (*regfile_test)(CudaBackend*, int device, const b2dp_compute_test_opts* opts,
+                        std::vector<b2dp_compute_test_result>& out, std::string& err) = nullptr;
 };
 DiagHooks& diag_hooks();  // ctx.cpp
 
