@@ -270,10 +270,10 @@ typedef struct b2dp_probe_result {
                                       last b2dp_probe_reset) => Unhealthy, sticky */
 #define B2DP_RES_MEMTEST 0x200u    /* a b2dp_memtest of this device failed or timed out since open (or the last
                                       b2dp_probe_reset) => Unhealthy, sticky */
-#define B2DP_RES_COMPUTE 0x400u    /* a compute, FP, SFU, shared-memory or register-file self-test (b2dp_compute_test,
-                                      b2dp_fp_test, b2dp_sfu_test, b2dp_smem_test, b2dp_regfile_test) of this device
-                                      failed or timed out since open (or the last b2dp_probe_reset) => Unhealthy,
-                                      sticky */
+#define B2DP_RES_COMPUTE 0x400u    /* a compute, FP, SFU, shared-memory, register-file or integer self-test
+                                      (b2dp_compute_test, b2dp_fp_test, b2dp_sfu_test, b2dp_smem_test,
+                                      b2dp_regfile_test, b2dp_int_test) of this device failed or timed out since open
+                                      (or the last b2dp_probe_reset) => Unhealthy, sticky */
 
 /* Replaces the exporter round trip getGPUHealth (exporter/health.go:42-82) and the evidence behind simpleHealthCheck
  * (plugin.go:161-206): launch the probe on every GPU of the context concurrently (one worker thread + stream per
@@ -285,7 +285,7 @@ B2DP_API int b2dp_probe_health(b2dp_ctx *ctx, const b2dp_probe_opts *opts, b2dp_
  * event numbered `mask` for `device` (seen by contexts opened with xid=1).  The reference has no equivalent. */
 B2DP_API int b2dp_probe_inject_fault(b2dp_ctx *ctx, int device, uint64_t word_index, uint32_t mask);
 /* Re-fill the probe buffers of `device` (-1 = all) with a clean pattern; also clears a latched Xid, a latched memtest
- * failure and a latched compute-, FP-, SFU-, shared-memory- or register-file-test failure. */
+ * failure and a latched compute-, FP-, SFU-, shared-memory-, register-file- or integer-test failure. */
 B2DP_API int b2dp_probe_reset(b2dp_ctx *ctx, int device);
 /* Set the bandwidth ceiling (gbs_ref) of `device` (-1 = all) the fractional floor refers to, e.g. to the site's measured
  * HBM peak; gbs_ref <= 0 restores the device's own calibration.  Also how tests move a device across the 0.8 line. */
@@ -500,6 +500,26 @@ B2DP_API int b2dp_smem_test(b2dp_ctx *ctx, int device, const b2dp_compute_test_o
  * backend with the in-process probe only; B2DP_E_UNSUPPORTED otherwise. */
 B2DP_API int b2dp_regfile_test(b2dp_ctx *ctx, int device, const b2dp_compute_test_opts *opts,
                                b2dp_compute_test_result *out, int cap, int *n);
+
+/* ---- on-demand integer and warp-exchange self-test (same opts, result and latch as the tensor-core self-test) ---- */
+#define B2DP_IT_MAD 0              /* b2dp_int_test's format index: multiplier, adder and carries, dp4a */
+#define B2DP_IT_BIT 1              /* logic, shifter, bit-count units, byte permute, compare */
+#define B2DP_IT_WARP 2             /* the lane-exchange network: shfl, vote, redux, match */
+
+/* An on-demand check of every SM's integer pipes and warp-exchange network on `device` (-1 = every GPU, concurrently
+ * on their workers): evidence behind the per-GPU verdict the exporter round trip supplies in the reference
+ * (exporter/health.go:42-82), merged the same way (exporter/health.go:86-106) through the sticky B2DP_RES_COMPUTE bit.
+ * int_selftest.cuh fills every SM with CTAs of 128 threads; every thread runs each op of the format, as inline PTX, on
+ * 20 / 12 / 12 operand sets that hold every crafted class next to random words: mad.lo, mul.hi, mad.wide, the carry
+ * pairs and dp4a (B2DP_IT_MAD); lop3, shf, shr, shl, popc, clz, bfind, brev, prmt, min / max and sad (B2DP_IT_BIT);
+ * shfl.sync in its four modes at segment widths 32, 16 and 8, vote.ballot, redux.sync, match.any and match.all with
+ * the full member mask (B2DP_IT_WARP).  All of it is two's-complement arithmetic or a lane permutation, so the host
+ * computes every result word exactly; every thread's fold of its result words must equal the host's check value.
+ * tflops[] is T result words/s.  Verdict, latching, the probe lock, the busy skip, the deadline and the release of
+ * every allocation are exactly b2dp_compute_test's.  cuda: backend with the in-process probe only;
+ * B2DP_E_UNSUPPORTED otherwise. */
+B2DP_API int b2dp_int_test(b2dp_ctx *ctx, int device, const b2dp_compute_test_opts *opts,
+                           b2dp_compute_test_result *out, int cap, int *n);
 
 /* exporter/health.go:86-106 PopulatePerGPUDHealth(devs, defaultHealth) merge rule.
  * have_source = 0 reproduces "exporter socket absent / RPC failed" (every device gets the

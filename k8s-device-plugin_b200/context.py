@@ -63,7 +63,8 @@ class ComputeTestResult:
     first_bad_tile: int
     ms: List[float]
     tflops: List[float]            # 2 M N K x result tiles compared / ms (TOPS for INT8; fp_test: 2 x FMAs / ms;
-                                   # sfu_test: MUFU results / ms, in T results/s; smem_test, regfile_test: TB/s)
+                                   # sfu_test: MUFU results / ms, in T results/s; smem_test, regfile_test: TB/s;
+                                   # int_test: result words / ms, in T results/s)
 
     def bad_sms(self) -> List[int]:
         return [s for s in range(256) if (self.bad_sm_mask[s // 64] >> (s % 64)) & 1]
@@ -282,6 +283,22 @@ class Context:
         opts = N.ComputeTestOpts(duration_ms, timeout_ms, N.CT_EVEN_IF_BUSY if even_if_busy else 0, fault_sm, fault_mask, 0)
         rc, arr, n = N.grow_call(lambda cap: (N.ComputeTestResult * cap)(),
                                  lambda a, cap, pn: N.lib.b2dp_regfile_test(self._h, device, C.byref(opts), a, cap, pn))
+        N.check(rc, self._h)
+        return [ComputeTestResult(r.device, bool(r.healthy), r.err, r.flags, r.seed, r.sm_count, r.nsmid, r.sms_covered,
+                                  list(r.bad_sm_mask), list(r.mismatches), r.first_bad_sm, r.first_bad_format,
+                                  r.first_bad_tile, list(r.ms), list(r.tflops)) for r in arr[:n]]
+
+    def int_test(self, device: int = -1, duration_ms: int = 0, timeout_ms: int = 0, even_if_busy: bool = False,
+                 fault_sm: int = -1, fault_mask: int = 0) -> List[ComputeTestResult]:
+        """On-demand integer and warp-exchange self-test of `device` (-1 = every GPU, b2dp_int_test): every SM's integer
+        pipes (multiplier, adder and carries, logic, shifter, bit counts, byte permute, compare) and its shuffle / vote /
+        redux / match network against results the host computed exactly, for duration_ms per format (0 = 1000).  The
+        per-format lists are indexed by IT_MAD, IT_BIT, IT_WARP; tflops holds T result words/s.  A failure is latched
+        like compute_test()'s (RES_COMPUTE until probe_reset()); fault_sm / fault_mask flips bits of one result word of
+        one thread of the SM with that %smid, in the first comparison."""
+        opts = N.ComputeTestOpts(duration_ms, timeout_ms, N.CT_EVEN_IF_BUSY if even_if_busy else 0, fault_sm, fault_mask, 0)
+        rc, arr, n = N.grow_call(lambda cap: (N.ComputeTestResult * cap)(),
+                                 lambda a, cap, pn: N.lib.b2dp_int_test(self._h, device, C.byref(opts), a, cap, pn))
         N.check(rc, self._h)
         return [ComputeTestResult(r.device, bool(r.healthy), r.err, r.flags, r.seed, r.sm_count, r.nsmid, r.sms_covered,
                                   list(r.bad_sm_mask), list(r.mismatches), r.first_bad_sm, r.first_bad_format,
