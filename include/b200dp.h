@@ -270,10 +270,10 @@ typedef struct b2dp_probe_result {
                                       last b2dp_probe_reset) => Unhealthy, sticky */
 #define B2DP_RES_MEMTEST 0x200u    /* a b2dp_memtest of this device failed or timed out since open (or the last
                                       b2dp_probe_reset) => Unhealthy, sticky */
-#define B2DP_RES_COMPUTE 0x400u    /* a compute, FP, SFU, shared-memory, register-file or integer self-test
+#define B2DP_RES_COMPUTE 0x400u    /* a compute, FP, SFU, shared-memory, register-file, integer or L2 self-test
                                       (b2dp_compute_test, b2dp_fp_test, b2dp_sfu_test, b2dp_smem_test,
-                                      b2dp_regfile_test, b2dp_int_test) of this device failed or timed out since open
-                                      (or the last b2dp_probe_reset) => Unhealthy, sticky */
+                                      b2dp_regfile_test, b2dp_int_test, b2dp_l2_test) of this device failed or timed
+                                      out since open (or the last b2dp_probe_reset) => Unhealthy, sticky */
 
 /* Replaces the exporter round trip getGPUHealth (exporter/health.go:42-82) and the evidence behind simpleHealthCheck
  * (plugin.go:161-206): launch the probe on every GPU of the context concurrently (one worker thread + stream per
@@ -285,7 +285,7 @@ B2DP_API int b2dp_probe_health(b2dp_ctx *ctx, const b2dp_probe_opts *opts, b2dp_
  * event numbered `mask` for `device` (seen by contexts opened with xid=1).  The reference has no equivalent. */
 B2DP_API int b2dp_probe_inject_fault(b2dp_ctx *ctx, int device, uint64_t word_index, uint32_t mask);
 /* Re-fill the probe buffers of `device` (-1 = all) with a clean pattern; also clears a latched Xid, a latched memtest
- * failure and a latched compute-, FP-, SFU-, shared-memory-, register-file- or integer-test failure. */
+ * failure and a latched compute-, FP-, SFU-, shared-memory-, register-file-, integer- or L2-test failure. */
 B2DP_API int b2dp_probe_reset(b2dp_ctx *ctx, int device);
 /* Set the bandwidth ceiling (gbs_ref) of `device` (-1 = all) the fractional floor refers to, e.g. to the site's measured
  * HBM peak; gbs_ref <= 0 restores the device's own calibration.  Also how tests move a device across the 0.8 line. */
@@ -520,6 +520,26 @@ B2DP_API int b2dp_regfile_test(b2dp_ctx *ctx, int device, const b2dp_compute_tes
  * B2DP_E_UNSUPPORTED otherwise. */
 B2DP_API int b2dp_int_test(b2dp_ctx *ctx, int device, const b2dp_compute_test_opts *opts,
                            b2dp_compute_test_result *out, int cap, int *n);
+
+/* ---- on-demand L2 self-test (same opts, result and latch as the tensor-core self-test) ---- */
+#define B2DP_L2_WORD 0             /* b2dp_l2_test's format index: March C- over an L2-resident span, 16-byte accesses */
+#define B2DP_L2_BYTE 1             /* the same span with byte and half-word stores, 16-byte reads */
+#define B2DP_L2_ATOM 2             /* the L2's atomic and reduction units on a hot block every CTA shares */
+
+/* An on-demand check of the L2 on `device` (-1 = every GPU, concurrently on their workers): evidence behind the
+ * per-GPU verdict the exporter round trip supplies in the reference (exporter/health.go:42-82), merged the same way
+ * (exporter/health.go:86-106) through the sticky B2DP_RES_COMPUTE bit.  l2_selftest.cuh runs every resident CTA of
+ * 128 threads as one cooperative grid.  B2DP_L2_WORD / B2DP_L2_BYTE march a span of 3/8 of the device's L2 (one of
+ * four windows of a buffer, per round) with ld/st.global.cg, and the slice of the span a CTA owns moves to another CTA
+ * at every element, behind a grid barrier: every value read must equal the pattern, and every thread's fold must
+ * equal the host's check.  B2DP_L2_ATOM drives atom add / inc / dec / exch / cas.b32 / cas.b64 and red and / or / xor
+ * / min / max / add.u64 / add.f32 / add.f64 / add.f16x2 / add.bf16x2 / v4.f32 on per-lane words; a rotating checker
+ * compares every final value with the host's order-free result and the returns with the host's multiset folds.
+ * tflops[] is TB/s for WORD and BYTE, and G atomic ops/s for ATOM.  Verdict, latching, the probe lock, the busy skip,
+ * the deadline, NVML's ECC totals and the release of every allocation are b2dp_smem_test's.  cuda: backend with the
+ * in-process probe on a device with cooperative launch only; B2DP_E_UNSUPPORTED otherwise. */
+B2DP_API int b2dp_l2_test(b2dp_ctx *ctx, int device, const b2dp_compute_test_opts *opts,
+                          b2dp_compute_test_result *out, int cap, int *n);
 
 /* exporter/health.go:86-106 PopulatePerGPUDHealth(devs, defaultHealth) merge rule.
  * have_source = 0 reproduces "exporter socket absent / RPC failed" (every device gets the

@@ -37,6 +37,7 @@
 #include "pattern_math.hpp"
 #include "fp_selftest.cuh"
 #include "int_selftest.cuh"
+#include "l2_selftest.cuh"
 #include "rf_selftest.cuh"
 #include "sfu_selftest.cuh"
 #include "smem_selftest.cuh"
@@ -1576,11 +1577,11 @@ static int cuda_memtest(CudaBackend* be, int device, const b2dp_memtest_opts* op
 }
 
 // ---- on-demand compute self-tests (b2dp_compute_test, b2dp_fp_test, b2dp_sfu_test, b2dp_smem_test,
-// b2dp_regfile_test, b2dp_int_test) ------------------------------------------------------------------------------------
+// b2dp_regfile_test, b2dp_int_test, b2dp_l2_test) ---------------------------------------------------------------------
 // One launch per format on one GPU, on that GPU's worker: tc_selftest.cuh (tensor cores: BF16, FP8, INT8),
 // fp_selftest.cuh (FP32 FMA, FP64 FMA, FP64 tensor cores), sfu_selftest.cuh (the special-function unit),
-// smem_selftest.cuh (shared memory and the SM-to-SM DSMEM path), rf_selftest.cuh (the register file) or int_selftest.cuh
-// (the integer pipes and the warp-exchange network).  The host builds
+// smem_selftest.cuh (shared memory and the SM-to-SM DSMEM path), rf_selftest.cuh (the register file), int_selftest.cuh
+// (the integer pipes and the warp-exchange network) or l2_selftest.cuh (the L2 and its atomic units).  The host builds
 // every operand table and every comparison value itself (compute_test_math.hpp, fp_test_math.hpp, smem_test_math.hpp,
 // rf_test_math.hpp, int_test_math.hpp): a health test must not ask the device under test for its own reference values.  The SFU test departs from that rule, because no
 // bit-level model of MUFU is published: its reference step (sfu_reference) runs one CTA on every SM, takes each result
@@ -1589,6 +1590,8 @@ static int cuda_memtest(CudaBackend* be, int device, const b2dp_memtest_opts* op
 // deadline, busy skip and the release of every allocation before the job ends, whatever happened -- through a
 // DiagSuite.
 constexpr uint32_t kComputeTestDefaultMs = 1000;
+constexpr int kDiagScratchHeaderWords = 64;  // DiagSuite::scratch's header
+static_assert(kL2HdrWords == kDiagScratchHeaderWords, "l2_selftest's scratch header is the driver's");
 
 using CtKernel = void (*)(const uint8_t*, const uint32_t*, unsigned long long, int, uint32_t, CtRecord*,
                           unsigned long long, uint32_t*);
@@ -1615,7 +1618,7 @@ struct DiagSuite {
     const uint32_t* smem;                      // dynamic shared memory per format
     const uint32_t* table_bytes;               // bytes of one tile's table per format
     void (*build_tile)(uint32_t seed, int fmt, int tile, uint8_t* table, uint32_t* check);
-    double (*macs_per_tile)(int fmt);          // multiply-adds of one comparison
+    double (*macs_per_tile)(int fmt);          // multiply-adds of one comparison (null with `scratch`: it sets them)
     bool per_device_seed;                      // seed ^ (device << 16) per GPU, tables built on each worker; else one
                                                // seed and one set of tables per call
     // Optional step on the worker before the timed launches (the SFU test's reference launch; null for the tensor and
@@ -1630,6 +1633,13 @@ struct DiagSuite {
     cudaError_t (*size_grid)(Gpu* g, int fmt, int* grid, const char** where);
     bool ecc;                                  // read NVML's volatile ECC totals around the timed launches
     const char* test_name;                     // in the error of a backend without the test; null: by the fields above
+    // Optional per-format device scratch buffer (the L2 test's spans and hot block; null: none): its size in bytes
+    // for `grid` CTAs, the kDiagScratchHeaderWords header words copied to its start (the rest is zeroed), and the
+    // per-CTA multiply-adds of one comparison, which depend on the buffer's size and take macs_per_tile's place.  Its
+    // pointer is the kernel's last argument; it is allocated and released with the other buffers.
+    cudaError_t (*scratch)(Gpu* g, int fmt, int grid, size_t* bytes, uint32_t* header, double* macs_per_cta,
+                           const char** where);
+    bool cooperative;                          // launch with cudaLaunchCooperativeKernel (every CTA co-resident)
 };
 
 static void ct_suite_tile(uint32_t seed, int fmt, int tile, uint8_t* table, uint32_t* check) {
@@ -1831,6 +1841,65 @@ static const DiagSuite kIntSuite = {"integer test", "int_selftest", "mad/bit/war
                                     it_suite_tile, it_suite_half_results, false, nullptr,
                                     "%.2f/%.2f/%.2f T results/s", nullptr, false, "integer self-test"};
 
+// ---- the L2 test's suite ----
+static const CtKernel kL2Kernels[kL2Formats] = {l2_selftest<L2_WORD, false>, l2_selftest<L2_BYTE, false>,
+                                                l2_selftest<L2_ATOM, false>};
+static const uint32_t kL2Smem[kL2Formats] = {0, 0, 0};
+static const uint32_t kL2TableBytes[kL2Formats] = {l2_table_bytes(L2_WORD), l2_table_bytes(L2_BYTE),
+                                                   l2_table_bytes(L2_ATOM)};
+static void l2_suite_tile(uint32_t seed, int fmt, int tile, uint8_t* table, uint32_t* check) {
+    l2_build_tile(seed, fmt, tile, reinterpret_cast<uint32_t*>(table), check);
+}
+
+// Every resident CTA, launched cooperatively: the grid barrier needs them all at once.
+static cudaError_t l2_size_grid(Gpu* g, int fmt, int* grid, const char** where) {
+    int dev = 0, coop = 0, per_sm = 0;
+    cudaError_t ce = cudaGetDevice(&dev);
+    if (ce == cudaSuccess) ce = cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev);
+    if (ce != cudaSuccess) { *where = "cudaDeviceGetAttribute(cudaDevAttrCooperativeLaunch)"; return ce; }
+    if (!coop) {
+        *where = "l2_selftest: the device has no cooperative launch (cudaDevAttrCooperativeLaunch = 0), which the "
+                 "grid barrier needs";
+        return cudaErrorNotSupported;
+    }
+    if ((ce = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kL2Kernels[fmt], kCtThreads, 0)) != cudaSuccess) {
+        *where = "cudaOccupancyMaxActiveBlocksPerMultiprocessor(l2_selftest)";
+        return ce;
+    }
+    *grid = (int)g->sms * (per_sm > 0 ? per_sm : 1);
+    if (*grid > kL2MaxCtas) { *where = "l2_selftest: more resident CTAs than its fold slots"; return cudaErrorInvalidConfiguration; }
+    return cudaSuccess;
+}
+
+// WORD / BYTE: kL2Windows spans of 3/8 of the L2 each; ATOM: the hot block.  The rate's numerator depends on the span:
+// *half is half of each CTA's share of one comparison's bytes (ATOM: ops x 1e3), as tflops[] = 2 x it x comparisons / ms.
+static cudaError_t l2_scratch(Gpu* g, int fmt, int grid, size_t* bytes, uint32_t* header, double* half,
+                              const char** where) {
+    int dev = 0, l2 = 0;
+    cudaError_t ce = cudaGetDevice(&dev);
+    if (ce == cudaSuccess) ce = cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, dev);
+    if (ce != cudaSuccess) { *where = "cudaDeviceGetAttribute(cudaDevAttrL2CacheSize)"; return ce; }
+    size_t data = kL2AtomHotWords * 4ull;
+    if (fmt != L2_ATOM) {
+        const uint32_t K = l2_span_blocks(l2_default_span((unsigned long long)l2), grid);
+        header[kL2HdrBlocks] = K;
+        data = (size_t)kL2Windows * K * grid * kL2BlockBytes;
+        // tflops[] = 2 x this x comparisons / ms, and every CTA counts each comparison: TB/s of L2 traffic
+        *half = 0.5 * l2_bytes_per_comparison(fmt, (double)K * grid * kL2BlockBytes) / grid;
+        logf(0, "%s L2 test: %d CTAs, span %.2f MiB of a %d KiB L2", g->dev.id.c_str(), grid,
+             (double)K * grid * kL2BlockBytes / (1 << 20), l2 >> 10);
+    } else {
+        // G ops/s (x 1e3 against the T of the other two): 20 atomics per thread per comparison, a v4 op counts once
+        *half = 0.5 * kCtThreads * 20 * 1e3;
+    }
+    *bytes = (size_t)kL2DataOff * 4 + data;
+    return cudaSuccess;
+}
+
+static const DiagSuite kL2Suite = {"L2 test", "l2_selftest", "word/byte/atom", kL2Kernels, kL2Smem, kL2TableBytes,
+                                   l2_suite_tile, nullptr, false, nullptr, "%.2f/%.2f/%.2f TB/s, TB/s, G ops/s",
+                                   l2_size_grid, true, "L2 self-test", l2_scratch, true};
+
 static std::shared_ptr<DiagTables> diag_build_tables(const DiagSuite& su, uint32_t seed) {
     auto t = std::make_shared<DiagTables>();
     for (int f = 0; f < kCtFormats; ++f) {
@@ -1849,6 +1918,7 @@ static void compute_test_one(const DiagSuite& su, CudaBackend* be, Gpu* g, const
                              std::string* err) {
     uint8_t* img[kCtFormats] = {};
     uint32_t* chk[kCtFormats] = {};
+    uint32_t* scr[kCtFormats] = {};
     CtRecord* rec_h = nullptr;
     CtRecord* rec_d = nullptr;
     cudaEvent_t ev[kCtFormats + 1] = {};
@@ -1860,6 +1930,7 @@ static void compute_test_one(const DiagSuite& su, CudaBackend* be, Gpu* g, const
         for (int f = 0; f < kCtFormats; ++f) {
             if (img[f]) cudaFree(img[f]);
             if (chk[f]) cudaFree(chk[f]);
+            if (scr[f]) cudaFree(scr[f]);
         }
         if (rec_h) cudaFreeHost(rec_h);
         for (cudaEvent_t e : ev)
@@ -1869,6 +1940,9 @@ static void compute_test_one(const DiagSuite& su, CudaBackend* be, Gpu* g, const
     {
         probe_flush(g);  // an armed heartbeat pass must not run underneath
         int grid[kCtFormats], off[kCtFormats + 1] = {0};
+        double macs[kCtFormats] = {};  // per comparison: from macs_per_tile, or from scratch() once it is sized
+        if (su.macs_per_tile)
+            for (int f = 0; f < kCtFormats; ++f) macs[f] = su.macs_per_tile(f);
         for (int f = 0; f < kCtFormats; ++f) {
             CT_TRY(cudaFuncSetAttribute(su.kernels[f], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)su.smem[f]));
             CT_TRY(cudaFuncSetAttribute(su.kernels[f], cudaFuncAttributePreferredSharedMemoryCarveout, 100));
@@ -1903,6 +1977,14 @@ static void compute_test_one(const DiagSuite& su, CudaBackend* be, Gpu* g, const
             CT_TRY(cudaMalloc(&chk[f], checks.size() * sizeof(uint32_t)));
             CT_TRY(cudaMemcpy(img[f], tables.data(), tables.size(), cudaMemcpyHostToDevice));
             CT_TRY(cudaMemcpy(chk[f], checks.data(), checks.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+            if (su.scratch) {
+                size_t bytes = 0;
+                uint32_t header[kDiagScratchHeaderWords] = {};
+                if ((ce = su.scratch(g, f, grid[f], &bytes, header, &macs[f], &where)) != cudaSuccess) goto done;
+                CT_TRY(cudaMalloc(&scr[f], bytes));
+                CT_TRY(cudaMemset(scr[f], 0, bytes));
+                CT_TRY(cudaMemcpy(scr[f], header, sizeof header, cudaMemcpyHostToDevice));
+            }
         }
         for (cudaEvent_t& e : ev) CT_TRY(cudaEventCreate(&e));
         // Device-wide counters, as the memory test reads them: a single-bit defect ECC corrects never reaches the data
@@ -1914,9 +1996,22 @@ static void compute_test_one(const DiagSuite& su, CudaBackend* be, Gpu* g, const
 
         CT_TRY(cudaEventRecord(ev[0], g->stream));
         for (int f = 0; f < kCtFormats; ++f) {
-            su.kernels[f]<<<grid[f], kCtThreads, su.smem[f], g->stream>>>(
-                img[f], chk[f], (unsigned long long)duration_ms * 1000000ull, o.fault_sm, o.fault_mask, rec_d + off[f],
-                (unsigned long long)(f + 1), nullptr);
+            if (su.cooperative) {
+                const uint8_t* a_img = img[f];
+                const uint32_t* a_chk = chk[f];
+                unsigned long long a_ns = (unsigned long long)duration_ms * 1000000ull, a_seq = (unsigned long long)(f + 1);
+                int a_sm = o.fault_sm;
+                uint32_t a_mask = o.fault_mask;
+                CtRecord* a_rec = rec_d + off[f];
+                uint32_t* a_scr = scr[f];
+                void* args[] = {&a_img, &a_chk, &a_ns, &a_sm, &a_mask, &a_rec, &a_seq, &a_scr};
+                CT_TRY(cudaLaunchCooperativeKernel((const void*)su.kernels[f], dim3(grid[f]), dim3(kCtThreads), args,
+                                                   su.smem[f], g->stream));
+            } else {
+                su.kernels[f]<<<grid[f], kCtThreads, su.smem[f], g->stream>>>(
+                    img[f], chk[f], (unsigned long long)duration_ms * 1000000ull, o.fault_sm, o.fault_mask,
+                    rec_d + off[f], (unsigned long long)(f + 1), scr[f]);
+            }
             CT_TRY(cudaGetLastError());
             CT_TRY(cudaEventRecord(ev[f + 1], g->stream));
         }
@@ -1974,7 +2069,7 @@ static void compute_test_one(const DiagSuite& su, CudaBackend* be, Gpu* g, const
                 r->first_bad_sm = bad_sm;
                 r->first_bad_tile = bad_tile;
             }
-            if (r->ms[f] > 0) r->tflops[f] = (float)(2.0 * su.macs_per_tile(f) * (double)compared / r->ms[f] * 1e-9);
+            if (r->ms[f] > 0) r->tflops[f] = (float)(2.0 * macs[f] * (double)compared / r->ms[f] * 1e-9);
         }
         for (int s = 0; s < kCtMaxSmId; ++s) r->sms_covered += seen[0][s] && seen[1][s] && seen[2][s];
         if (r->sms_covered < r->sm_count) r->flags |= B2DP_CT_PARTIAL_COVERAGE;
@@ -2092,6 +2187,11 @@ static int cuda_int_test(CudaBackend* be, int device, const b2dp_compute_test_op
     return cuda_diag_test(kIntSuite, be, device, opts, out, err);
 }
 
+static int cuda_l2_test(CudaBackend* be, int device, const b2dp_compute_test_opts* opts,
+                        std::vector<b2dp_compute_test_result>& out, std::string& err) {
+    return cuda_diag_test(kL2Suite, be, device, opts, out, err);
+}
+
 static bool cuda_diag_latched(CudaBackend* be) {
     for (auto& g : be->gpus)
         if (g->memtest_fault.load() || g->compute_fault.load()) return true;
@@ -2101,7 +2201,7 @@ static bool cuda_diag_latched(CudaBackend* be) {
 // registered when the library is loaded, before any entry point can run (internal.hpp DiagHooks)
 [[maybe_unused]] static const bool kDiagRegistered = [] {
     diag_hooks() = DiagHooks{cuda_memtest, cuda_compute_test, cuda_fp_test, cuda_diag_latched, cuda_sfu_test,
-                             cuda_smem_test, cuda_regfile_test, cuda_int_test};
+                             cuda_smem_test, cuda_regfile_test, cuda_int_test, cuda_l2_test};
     return true;
 }();
 

@@ -64,6 +64,8 @@ struct Flags {
                                                      // shared-memory test), for compute_test_ms per format
     int int_test_at_start = 0;                       // likewise for the integer and warp-exchange self-test (after the
                                                      // register-file test), for compute_test_ms per format
+    int l2_test_at_start = 0;                        // likewise for the L2 self-test (after the integer test), for
+                                                     // compute_test_ms per format
     bool version = false;
     bool labels_mode = false, reconcile = false, patch = false;
     std::string labels;                              // csv of generator names, or "all"
@@ -108,6 +110,7 @@ bool parse_flags(int argc, char** argv, Flags& f, std::string& err) {
         else if (name == "smem_test_at_start") f.smem_test_at_start = atoi(val.c_str());
         else if (name == "regfile_test_at_start") f.regfile_test_at_start = atoi(val.c_str());
         else if (name == "int_test_at_start") f.int_test_at_start = atoi(val.c_str());
+        else if (name == "l2_test_at_start") f.l2_test_at_start = atoi(val.c_str());
         else if (name == "labels") { f.labels_mode = true; f.labels = val; }
         else { err = "flag provided but not defined: -" + name; return false; }
     }
@@ -682,6 +685,32 @@ void run_int_test(b2dp_ctx* ctx, const Flags& fl) {
     }
 }
 
+// -l2_test_at_start=1: likewise for the L2 self-test (a march over an L2-resident span that moves between SMs, and
+// the L2 atomic units, against host values), after the integer test, for -compute_test_ms per format.
+void run_l2_test(b2dp_ctx* ctx, const Flags& fl) {
+    b2dp_compute_test_opts o{};
+    o.duration_ms = fl.compute_test_ms;
+    o.fault_sm = -1;
+    if (fl.l2_test_at_start >= 2) o.flags |= B2DP_CT_EVEN_IF_BUSY;
+    b2dp_compute_test_result res[64];
+    int n = 0;
+    const int rc = b2dp_l2_test(ctx, -1, &o, res, 64, &n);
+    if (rc != B2DP_OK) {
+        logf("L2 test at start not run: %s (%s)", b2dp_strerror(rc), b2dp_last_error(ctx));
+        return;
+    }
+    std::vector<b2dp_device> devs(n > 0 ? n : 1);
+    int nd = 0;
+    if (b2dp_enumerate(ctx, devs.data(), (int)devs.size(), &nd) != B2DP_OK) nd = 0;
+    for (int i = 0; i < n; ++i) {
+        const b2dp_compute_test_result& r = res[i];
+        logf("L2 test %s: %s, flags 0x%x, SMs %d/%d, mismatches %llu/%llu/%llu, first bad SM %d, %.2f/%.2f/%.2f "
+             "TB/s, TB/s, G ops/s", r.device < nd ? devs[r.device].id : "?", r.healthy ? "Healthy" : "Unhealthy", r.flags,
+             r.sms_covered, r.sm_count, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
+             (unsigned long long)r.mismatches[2], r.first_bad_sm, r.tflops[0], r.tflops[1], r.tflops[2]);
+    }
+}
+
 }  // namespace
 
 int main(int argc, char** argv) {
@@ -719,6 +748,7 @@ int main(int argc, char** argv) {
     if (fl.smem_test_at_start) run_smem_test(ctx, fl);
     if (fl.regfile_test_at_start) run_regfile_test(ctx, fl);
     if (fl.int_test_at_start) run_int_test(ctx, fl);
+    if (fl.l2_test_at_start) run_l2_test(ctx, fl);
     char names[64][64];
     int n_res = 0;
     rc = b2dp_resource_list(ctx, fl.strategy.c_str(), names, 64, &n_res);  // main.go:141-146
