@@ -274,6 +274,8 @@ typedef struct b2dp_probe_result {
                                       (b2dp_compute_test, b2dp_fp_test, b2dp_sfu_test, b2dp_smem_test,
                                       b2dp_regfile_test, b2dp_int_test, b2dp_l2_test) of this device failed or timed
                                       out since open (or the last b2dp_probe_reset) => Unhealthy, sticky */
+#define B2DP_RES_HOSTLINK 0x800u   /* a b2dp_hostlink_test of this device failed or timed out since open (or the last
+                                      b2dp_probe_reset) => Unhealthy, sticky */
 
 /* Replaces the exporter round trip getGPUHealth (exporter/health.go:42-82) and the evidence behind simpleHealthCheck
  * (plugin.go:161-206): launch the probe on every GPU of the context concurrently (one worker thread + stream per
@@ -285,7 +287,8 @@ B2DP_API int b2dp_probe_health(b2dp_ctx *ctx, const b2dp_probe_opts *opts, b2dp_
  * event numbered `mask` for `device` (seen by contexts opened with xid=1).  The reference has no equivalent. */
 B2DP_API int b2dp_probe_inject_fault(b2dp_ctx *ctx, int device, uint64_t word_index, uint32_t mask);
 /* Re-fill the probe buffers of `device` (-1 = all) with a clean pattern; also clears a latched Xid, a latched memtest
- * failure and a latched compute-, FP-, SFU-, shared-memory-, register-file-, integer- or L2-test failure. */
+ * failure, a latched compute-, FP-, SFU-, shared-memory-, register-file-, integer- or L2-test failure and a latched
+ * host-link-test failure. */
 B2DP_API int b2dp_probe_reset(b2dp_ctx *ctx, int device);
 /* Set the bandwidth ceiling (gbs_ref) of `device` (-1 = all) the fractional floor refers to, e.g. to the site's measured
  * HBM peak; gbs_ref <= 0 restores the device's own calibration.  Also how tests move a device across the 0.8 line. */
@@ -540,6 +543,75 @@ B2DP_API int b2dp_int_test(b2dp_ctx *ctx, int device, const b2dp_compute_test_op
  * in-process probe on a device with cooperative launch only; B2DP_E_UNSUPPORTED otherwise. */
 B2DP_API int b2dp_l2_test(b2dp_ctx *ctx, int device, const b2dp_compute_test_opts *opts,
                           b2dp_compute_test_result *out, int cap, int *n);
+
+/* ---- on-demand host-link self-test (feeds the same per-GPU verdict as the probe) ---- */
+typedef struct b2dp_hostlink_opts {
+    uint64_t bytes;          /* per buffer; 0 = 64 MiB; a multiple of 16 and <= 1 GiB, else B2DP_E_INVAL */
+    uint32_t duration_ms;    /* per format; 0 = 1000 (every format still runs at least one round) */
+    uint32_t timeout_ms;     /* per-call deadline; 0 = 10000 + 3 * duration */
+    uint32_t flags;          /* B2DP_HL_EVEN_IF_BUSY */
+    uint64_t fault_word;     /* test hook: in the first round of every format, XOR fault_mask into this word (H2D: of the
+                                device buffer the copy filled; D2H: of the device buffer about to be copied back; SM: as
+                                the SM reads it); ignored when fault_mask = 0 */
+    uint32_t fault_mask;
+    uint32_t reserved;
+} b2dp_hostlink_opts;
+#define B2DP_HL_EVEN_IF_BUSY 0x1u  /* test a GPU even while another process uses it (default: skip it) */
+
+#define B2DP_HL_H2D 0              /* format index: host -> device by copy engine, verified on the device */
+#define B2DP_HL_D2H 1              /* device -> host by copy engine, verified on the host */
+#define B2DP_HL_SM 2               /* the SMs read host memory and write host memory themselves (no copy engine) */
+typedef struct b2dp_hostlink_result {
+    int32_t device;             /* index into b2dp_enumerate() order */
+    int32_t healthy;            /* 1 Healthy, 0 Unhealthy (a failure is latched: B2DP_RES_HOSTLINK) */
+    int32_t err;                /* B2DP_OK | B2DP_E_CUDA | B2DP_E_TIMEOUT | B2DP_E_INVAL (fault_word outside the buffer) */
+    uint32_t flags;             /* B2DP_HL_* */
+    uint32_t seed;              /* pattern seed of the first round; each round advances it as the probe does */
+    int32_t sm_count;           /* the device's SM count */
+    int32_t sms_covered;        /* distinct SM ids that ran a CTA of the SM format */
+    int32_t host_numa_node;     /* the node the host buffers were bound to; -1 if they were not (B2DP_HL_NUMA_UNBOUND) */
+    uint64_t bad_sm_mask[4];    /* bit s: a CTA of the SM format on the SM with %smid s read a wrong word */
+    uint64_t rounds[3];         /* per format: rounds run */
+    uint64_t mismatches[3];     /* per format: wrong words its rounds found, device-side and host-side checks together
+                                   (a word wrong on the device is re-keyed and found again on the host) */
+    uint64_t first_bad_word[3]; /* per format: lowest wrong word index, UINT64_MAX if none */
+    uint64_t replays;           /* NVML PCIe replay counter delta over the call */
+    float ms[3];                /* per format: summed CUDA-event time of its transfers (H2D copies, D2H copies, SM
+                                   kernels) */
+    float gbs[3];               /* per format: bytes x rounds / ms (SM: 2 x bytes x rounds / ms, read plus written) */
+    int32_t link_gen;           /* highest PCIe generation NVML reported while a transfer was in flight; 0 if none */
+    int32_t link_width;         /* highest lane count likewise */
+    int32_t max_link_gen;       /* what the link and the device support (NVML); 0 if unknown */
+    int32_t max_link_width;
+    float link_gbs;             /* per-direction capacity of link_gen x link_width before packet overhead (Gen5 x16:
+                                   63.0) */
+    uint32_t reserved;
+} b2dp_hostlink_result;
+#define B2DP_HL_SKIPPED_BUSY 0x1u  /* another process uses the GPU: nothing ran, nothing latched; healthy = the last
+                                      heartbeat verdict */
+#define B2DP_HL_NUMA_UNBOUND 0x2u  /* the host buffers could not be bound to the GPU's NUMA node (reported, not failed) */
+#define B2DP_HL_LINK_NARROW 0x4u   /* link_width < max_link_width (reported, not failed) */
+#define B2DP_HL_LINK_SLOW 0x8u     /* link_gen < max_link_gen (reported, not failed) */
+#define B2DP_HL_REPLAYS 0x10u      /* the PCIe replay counter grew during the call (reported, not failed) */
+#define B2DP_HL_NO_NVML 0x20u      /* NVML gave no link generation, width or replay counter */
+
+/* An on-demand check of the path between host memory and the GPU on `device` (-1 = every GPU, concurrently on their
+ * workers): evidence behind the per-GPU verdict the exporter round trip supplies in the reference
+ * (exporter/health.go:42-82), merged the same way (exporter/health.go:86-106) through the sticky B2DP_RES_HOSTLINK bit.
+ * Two pinned host buffers of `bytes` are bound to the GPU's NUMA node, and every round moves the probe's pattern, with
+ * a new seed, across PCIe.  B2DP_HL_H2D and B2DP_HL_D2H run the same loop for duration_ms each: the host writes the
+ * pattern, a copy engine moves it to the device, hbm_probe_r128 verifies it there and re-keys it, a copy engine moves
+ * it back, and the host checks every word.  B2DP_HL_SM runs hostlink_selftest.cuh on every SM, which reads the host
+ * buffer and writes the other one directly, with 16- to 1-byte stores, and the host checks every word.  Healthy iff
+ * every CUDA call succeeded before the deadline, every format ran a round, every sequence number and record arrived,
+ * no check found a wrong word and every device checksum equals the host's closed form.  The PCIe link generation and
+ * width (sampled while transfers are in flight), their maxima and the replay counter come from NVML and are reported,
+ * never judged.  Every allocation is released before the call returns, on every path.  The probe lock is held
+ * throughout: a heartbeat waits for a running test.  A GPU another process uses is skipped (B2DP_HL_SKIPPED_BUSY)
+ * unless B2DP_HL_EVEN_IF_BUSY.  B2DP_E_INVAL for a bad `bytes`.  cuda: backend with the in-process probe only;
+ * B2DP_E_UNSUPPORTED otherwise. */
+B2DP_API int b2dp_hostlink_test(b2dp_ctx *ctx, int device, const b2dp_hostlink_opts *opts, b2dp_hostlink_result *out,
+                                int cap, int *n);
 
 /* exporter/health.go:86-106 PopulatePerGPUDHealth(devs, defaultHealth) merge rule.
  * have_source = 0 reproduces "exporter socket absent / RPC failed" (every device gets the

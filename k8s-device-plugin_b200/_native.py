@@ -53,6 +53,10 @@ RF_ALU, RF_LOAD, RF_HOLD = 0, 1, 2
 IT_MAD, IT_BIT, IT_WARP = 0, 1, 2
 L2_WORD, L2_BYTE, L2_ATOM = 0, 1, 2
 CT_ECC_CORRECTED, CT_ECC, CT_NO_ECC = 0x10, 0x20, 0x40
+RES_HOSTLINK = 0x800
+HL_EVEN_IF_BUSY = 1
+HL_H2D, HL_D2H, HL_SM = 0, 1, 2
+HL_SKIPPED_BUSY, HL_NUMA_UNBOUND, HL_LINK_NARROW, HL_LINK_SLOW, HL_REPLAYS, HL_NO_NVML = 1, 2, 4, 8, 0x10, 0x20
 
 Id64 = C.c_char * 64
 
@@ -147,6 +151,21 @@ class ComputeTestResult(C.Structure):
                 ("tflops", C.c_float * 3)]
 
 
+class HostlinkOpts(C.Structure):
+    _fields_ = [("bytes", C.c_uint64), ("duration_ms", C.c_uint32), ("timeout_ms", C.c_uint32), ("flags", C.c_uint32),
+                ("fault_word", C.c_uint64), ("fault_mask", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+class HostlinkResult(C.Structure):
+    _fields_ = [("device", C.c_int32), ("healthy", C.c_int32), ("err", C.c_int32), ("flags", C.c_uint32),
+                ("seed", C.c_uint32), ("sm_count", C.c_int32), ("sms_covered", C.c_int32),
+                ("host_numa_node", C.c_int32), ("bad_sm_mask", C.c_uint64 * 4), ("rounds", C.c_uint64 * 3),
+                ("mismatches", C.c_uint64 * 3), ("first_bad_word", C.c_uint64 * 3), ("replays", C.c_uint64),
+                ("ms", C.c_float * 3), ("gbs", C.c_float * 3), ("link_gen", C.c_int32), ("link_width", C.c_int32),
+                ("max_link_gen", C.c_int32), ("max_link_width", C.c_int32), ("link_gbs", C.c_float),
+                ("reserved", C.c_uint32)]
+
+
 if not os.path.exists(LIB_PATH):
     raise ImportError(
         "libb200dp.so is not built: run `python -c 'import __graft_entry__ as g; g.build()'` "
@@ -193,6 +212,7 @@ SIGNATURES = {
     "b2dp_regfile_test": (_i, [_vp, _i, _P(ComputeTestOpts), _P(ComputeTestResult), _i, _ip]),
     "b2dp_int_test": (_i, [_vp, _i, _P(ComputeTestOpts), _P(ComputeTestResult), _i, _ip]),
     "b2dp_l2_test": (_i, [_vp, _i, _P(ComputeTestOpts), _P(ComputeTestResult), _i, _ip]),
+    "b2dp_hostlink_test": (_i, [_vp, _i, _P(HostlinkOpts), _P(HostlinkResult), _i, _ip]),
     "b2dp_probe_set_ref": (_i, [_vp, _i, C.c_float]),
     "b2dp_probe_describe": (_i, [_vp, _i, _P(ProbeInfo)]),
     "b2dp_expected_checksum": (_i, [C.c_uint64, C.c_uint32, _P(C.c_uint64)]),

@@ -71,6 +71,33 @@ class ComputeTestResult:
 
 
 @dataclass
+class HostlinkResult:
+    device: int
+    healthy: bool
+    err: int
+    flags: int
+    seed: int
+    sm_count: int
+    sms_covered: int               # SM ids that ran a CTA of the SM format
+    host_numa_node: int            # -1: the host buffers were not bound (HL_NUMA_UNBOUND)
+    bad_sm_mask: List[int]         # 4 x 64 bits over %smid
+    rounds: List[int]              # per format: H2D, D2H, SM
+    mismatches: List[int]          # wrong words, device-side and host-side checks together
+    first_bad_word: List[int]      # 2^64 - 1 if none
+    replays: int                   # NVML PCIe replay counter delta
+    ms: List[float]                # summed event time of the transfers
+    gbs: List[float]               # bytes x rounds / ms (SM: read plus written)
+    link_gen: int                  # sampled while a transfer was in flight (0: NVML gave none)
+    link_width: int
+    max_link_gen: int
+    max_link_width: int
+    link_gbs: float                # per-direction capacity of link_gen x link_width
+
+    def bad_sms(self) -> List[int]:
+        return [s for s in range(256) if (self.bad_sm_mask[s // 64] >> (s % 64)) & 1]
+
+
+@dataclass
 class CycleStats:
     n_devices: int
     n_unhealthy: int
@@ -319,6 +346,24 @@ class Context:
         return [ComputeTestResult(r.device, bool(r.healthy), r.err, r.flags, r.seed, r.sm_count, r.nsmid, r.sms_covered,
                                   list(r.bad_sm_mask), list(r.mismatches), r.first_bad_sm, r.first_bad_format,
                                   r.first_bad_tile, list(r.ms), list(r.tflops)) for r in arr[:n]]
+
+    def hostlink_test(self, device: int = -1, bytes: int = 0, duration_ms: int = 0, timeout_ms: int = 0,
+                      even_if_busy: bool = False, fault_word: int = 0, fault_mask: int = 0) -> List[HostlinkResult]:
+        """On-demand host-link self-test of `device` (-1 = every GPU, b2dp_hostlink_test): the probe's pattern moved
+        between host buffers of `bytes` each (0 = 64 MiB) and the GPU by the copy engines (HL_H2D, HL_D2H) and by the
+        SMs' own loads and stores (HL_SM), for duration_ms per format (0 = 1000), every word checked against the
+        pattern on the side it arrived.  The PCIe link generation, width and replay count come from NVML, reported
+        only.  A failure is latched: later probe results carry RES_HOSTLINK and are Unhealthy until probe_reset().
+        fault_word / fault_mask is a test hook that flips bits of one word in the first round of every format."""
+        opts = N.HostlinkOpts(bytes, duration_ms, timeout_ms, N.HL_EVEN_IF_BUSY if even_if_busy else 0, fault_word,
+                              fault_mask, 0)
+        rc, arr, n = N.grow_call(lambda cap: (N.HostlinkResult * cap)(),
+                                 lambda a, cap, pn: N.lib.b2dp_hostlink_test(self._h, device, C.byref(opts), a, cap, pn))
+        N.check(rc, self._h)
+        return [HostlinkResult(r.device, bool(r.healthy), r.err, r.flags, r.seed, r.sm_count, r.sms_covered,
+                               r.host_numa_node, list(r.bad_sm_mask), list(r.rounds), list(r.mismatches),
+                               list(r.first_bad_word), r.replays, list(r.ms), list(r.gbs), r.link_gen, r.link_width,
+                               r.max_link_gen, r.max_link_width, r.link_gbs) for r in arr[:n]]
 
     # ---- ListAndWatch --------------------------------------------------------------------
     def list_and_watch(self, resource: str = "gpu", flags: int = N.LW_INITIAL, external: Optional[Dict[str, bool]] = None,

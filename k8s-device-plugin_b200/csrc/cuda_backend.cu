@@ -16,6 +16,9 @@
 #include <dlfcn.h>
 #include <pthread.h>
 #include <sched.h>
+#include <sys/mman.h>
+#include <sys/syscall.h>
+#include <unistd.h>
 
 #include <algorithm>
 #include <array>
@@ -31,6 +34,8 @@
 #include "gosem.hpp"
 #include "hbm_memtest.cuh"
 #include "hbm_probe.cuh"
+#include "hostlink_math.hpp"
+#include "hostlink_selftest.cuh"
 #include "internal.hpp"
 #include "memtest_math.hpp"
 #include "nvml_dyn.hpp"
@@ -109,6 +114,7 @@ struct Gpu {
     std::atomic<unsigned long long> xid_fault{0};  // first critical Xid seen on this device (sticky, like a real fault)
     std::atomic<bool> memtest_fault{false};        // a b2dp_memtest failed or timed out (sticky until b2dp_probe_reset)
     std::atomic<bool> compute_fault{false};        // a b2dp_compute_test or b2dp_fp_test failed or timed out (likewise)
+    std::atomic<bool> hostlink_fault{false};       // a b2dp_hostlink_test failed or timed out (likewise)
     int last_healthy = 1;
     // worker
     std::thread th;
@@ -1128,6 +1134,12 @@ int cuda_probe(CudaBackend* be, const b2dp_probe_opts* opts, std::vector<b2dp_pr
             out[i].healthy = 0;
             be->gpus[i]->last_healthy = 0;
         }
+    for (size_t i = 0; i < n; ++i)  // and a failed host-link self-test
+        if (be->gpus[i]->hostlink_fault.load(std::memory_order_relaxed)) {
+            out[i].flags |= B2DP_RES_HOSTLINK;
+            out[i].healthy = 0;
+            be->gpus[i]->last_healthy = 0;
+        }
     return B2DP_OK;
 }
 
@@ -1219,6 +1231,7 @@ int cuda_probe_reset(CudaBackend* be, int device, std::string& err) {
         g->xid_fault.store(0);  // operator acknowledgement: a latched Xid is cleared together with the buffers
         g->memtest_fault.store(false);  // and so is a failed memory test
         g->compute_fault.store(false);  // and a failed compute self-test
+        g->hostlink_fault.store(false);  // and a failed host-link self-test
         cudaError_t ce = cudaSuccess;
         run_sync(g, [&] {
             probe_flush(g);
@@ -2192,16 +2205,298 @@ static int cuda_l2_test(CudaBackend* be, int device, const b2dp_compute_test_opt
     return cuda_diag_test(kL2Suite, be, device, opts, out, err);
 }
 
+// ---- on-demand host-link self-test (b2dp_hostlink_test) ---------------------------------------------------------------
+// Host memory -> PCIe -> copy engines / SMs -> HBM and back, on the GPU's worker.  Two host buffers (Hs, the source the
+// host writes, and Hd, the destination the host checks) are mmap'd, bound to the GPU's NUMA node before their first
+// touch, touched, and registered as mapped pinned memory; two device buffers (A, B) of the same size take the copies.
+// Per round, with the probe's seed schedule:
+//   H2D, D2H: Hs <- pattern(s); A <- Hs (copy engine); hbm_probe_r128 verifies A and re-keys it into B; Hd <- B (copy
+//             engine); the host checks Hd against pattern(next).  The two formats run this loop for duration_ms each
+//             and differ in where the fault hook applies and which copy their rate times.
+//   SM:       Hs <- pattern(s); hostlink_sm reads Hs and writes Hd over the mapped pointers; the host checks Hd.
+// The link generation and width are sampled from NVML while a transfer is in flight (an idle link may train down).
+// Everything is released before the job ends, whatever happened.
+constexpr uint32_t kHostlinkDefaultMs = 1000;
+
+// Bind [p, p + len) to NUMA node `node` with the raw mbind syscall (MPOL_BIND); false if the kernel refuses.
+static bool hl_bind(void* p, size_t len, int node) {
+    constexpr int kMaxNodes = 1024, kMpolBind = 2;
+    constexpr int kBits = 8 * sizeof(unsigned long);
+    if (node < 0 || node >= kMaxNodes) return false;
+    unsigned long mask[kMaxNodes / kBits] = {};
+    mask[node / kBits] = 1ul << (node % kBits);
+    return syscall(SYS_mbind, p, len, kMpolBind, mask, (unsigned long)kMaxNodes + 1, 0u) == 0;
+}
+
+static void hostlink_one(CudaBackend* be, Gpu* g, const b2dp_hostlink_opts& o, unsigned long long bytes,
+                         uint32_t duration_ms, uint32_t timeout_ms, b2dp_hostlink_result* r, std::string* err) {
+    const size_t page = (size_t)sysconf(_SC_PAGESIZE);
+    const size_t len = (bytes + page - 1) / page * page;
+    const unsigned long long n_vec = bytes / 16, n_words = bytes / 4;
+    void* host[2] = {};                  // Hs, Hd (mmap)
+    bool registered[2] = {};
+    uint4* hdev[2] = {};                 // their device-mapped pointers
+    uint4* dbuf[2] = {};                 // A, B
+    ProbeCtl* ctl = nullptr;
+    ProbeOut* out_h = nullptr;
+    ProbeOut* out_d = nullptr;
+    HlRecord* rec_h = nullptr;
+    HlRecord* rec_d = nullptr;
+    cudaEvent_t ev[4] = {};
+    bool timed_out = false;
+    cudaError_t ce = cudaSuccess;
+    const char* where = "";
+    HlEvidence ev_;
+    auto release = [&] {  // every path ends here: nothing the test allocated outlives it
+        if (g->stream) cudaStreamSynchronize(g->stream);
+        for (int k = 0; k < 2; ++k) {
+            if (registered[k]) cudaHostUnregister(host[k]);
+            if (host[k]) munmap(host[k], len);
+            if (dbuf[k]) cudaFree(dbuf[k]);
+        }
+        if (ctl) cudaFree(ctl);
+        if (out_h) cudaFreeHost(out_h);
+        if (rec_h) cudaFreeHost(rec_h);
+        for (cudaEvent_t e : ev)
+            if (e) cudaEventDestroy(e);
+    };
+    // NVML: the link while a transfer is in flight (maximum over the samples), and the replay counter around the call
+    unsigned replays0 = 0, v = 0;
+    const bool nv = g->nvh != nullptr;
+    const bool have_replays = nv && be->nvml.pcie_replays && be->nvml.pcie_replays(g->nvh, &replays0) == 0;
+    if (nv && be->nvml.pcie_max_gen && be->nvml.pcie_max_gen(g->nvh, &v) == 0) r->max_link_gen = (int32_t)v;
+    if (nv && be->nvml.pcie_max_width && be->nvml.pcie_max_width(g->nvh, &v) == 0) r->max_link_width = (int32_t)v;
+    bool sampled = false;
+    auto sample = [&] {
+        unsigned gen = 0, width = 0;
+        if (!nv || !be->nvml.pcie_gen || !be->nvml.pcie_width) return;
+        if (be->nvml.pcie_gen(g->nvh, &gen) != 0 || be->nvml.pcie_width(g->nvh, &width) != 0) return;
+        sampled = true;
+        r->link_gen = std::max<int32_t>(r->link_gen, (int32_t)gen);
+        r->link_width = std::max<int32_t>(r->link_width, (int32_t)width);
+    };
+    const auto t_start = std::chrono::steady_clock::now();
+    const auto deadline = t_start + std::chrono::milliseconds(timeout_ms);
+    // wait for `e`, sampling the link meanwhile; false on a CUDA error (ce, where) or past the deadline (timed_out)
+    auto wait = [&](cudaEvent_t e, const char* what) {
+        for (;;) {
+            const cudaError_t q = cudaEventQuery(e);
+            if (q == cudaSuccess) return true;
+            if (q != cudaErrorNotReady) { ce = q; where = what; return false; }
+            sample();
+            if (std::chrono::steady_clock::now() > deadline) { timed_out = true; return false; }
+            std::this_thread::sleep_for(std::chrono::microseconds(100));
+        }
+    };
+    const bool inject = o.fault_mask != 0 && o.fault_word < n_words;
+    if (o.fault_mask && !inject) r->err = B2DP_E_INVAL;  // not injected; the test runs as it would without the hook
+#define HL_TRY(x) if ((ce = (x)) != cudaSuccess) { where = #x; goto done; }
+    {
+        probe_flush(g);  // an armed heartbeat pass must not run underneath
+        r->host_numa_node = g->dev.numa;
+        for (int k = 0; k < 2; ++k) {
+            void* p = mmap(nullptr, len, PROT_READ | PROT_WRITE, MAP_PRIVATE | MAP_ANONYMOUS, -1, 0);
+            if (p == MAP_FAILED) { ce = cudaErrorMemoryAllocation; where = "mmap (host buffer)"; goto done; }
+            host[k] = p;
+            if (!hl_bind(p, len, g->dev.numa)) r->host_numa_node = -1;  // before the first touch places the pages
+            memset(p, 0, len);
+            HL_TRY(cudaHostRegister(p, len, cudaHostRegisterMapped));
+            registered[k] = true;
+            HL_TRY(cudaHostGetDevicePointer((void**)&hdev[k], p, 0));
+            HL_TRY(cudaMalloc(&dbuf[k], bytes));
+        }
+        if (r->host_numa_node < 0) r->flags |= B2DP_HL_NUMA_UNBOUND;
+        HL_TRY(cudaMalloc(&ctl, sizeof(ProbeCtl)));
+        {
+            ProbeCtl init = {};
+            init.first_bad = ~0ull;
+            init.t_start_ns = ~0ull;
+            HL_TRY(cudaMemcpy(ctl, &init, sizeof init, cudaMemcpyHostToDevice));
+        }
+        HL_TRY(cudaHostAlloc(&out_h, sizeof(ProbeOut), cudaHostAllocMapped));
+        memset(out_h, 0, sizeof(ProbeOut));
+        HL_TRY(cudaHostGetDevicePointer(&out_d, out_h, 0));
+        int per_sm = 0;
+        HL_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, hostlink_sm<kHlThreads, kHlUnroll>, kHlThreads, 0));
+        const int grid = (int)g->sms * (per_sm > 0 ? per_sm : 1);  // every CTA resident at once: every SM runs one
+        HL_TRY(cudaHostAlloc(&rec_h, (size_t)grid * sizeof(HlRecord), cudaHostAllocMapped));
+        memset(rec_h, 0, (size_t)grid * sizeof(HlRecord));
+        HL_TRY(cudaHostGetDevicePointer(&rec_d, rec_h, 0));
+        for (cudaEvent_t& e : ev) HL_TRY(cudaEventCreate(&e));
+
+        const std::array<unsigned long long, 32>& bc = host_bitcounts(be, n_words);
+        uint32_t* hs = static_cast<uint32_t*>(host[0]);
+        const uint32_t* hd = static_cast<const uint32_t*>(host[1]);
+        std::vector<uint8_t> seen(kCtMaxSmId, 0);
+        uint32_t s = r->seed;
+        unsigned long long seq = 0;
+        for (int f = 0; f < kHlFormats; ++f) {
+            const auto t_fmt = std::chrono::steady_clock::now();
+            double ms_sum = 0.0;
+            r->first_bad_word[f] = ~0ull;
+            for (unsigned long long k = 0;; ++k) {
+                if (k > 0 && std::chrono::steady_clock::now() - t_fmt >= std::chrono::milliseconds(duration_ms)) break;
+                if (std::chrono::steady_clock::now() > deadline) { timed_out = true; goto done; }
+                const uint32_t next = hl_next_seed(s);
+                const bool poke = inject && k == 0;
+                hl_fill(hs, n_words, s);
+                ++seq;
+                float ms = 0.f;
+                if (f != B2DP_HL_SM) {
+                    HL_TRY(cudaEventRecord(ev[0], g->stream));
+                    HL_TRY(cudaMemcpyAsync(dbuf[0], hs, bytes, cudaMemcpyHostToDevice, g->stream));
+                    HL_TRY(cudaEventRecord(ev[1], g->stream));
+                    if (poke && f == B2DP_HL_H2D)
+                        hbm_poke<<<1, 1, 0, g->stream>>>(reinterpret_cast<uint32_t*>(dbuf[0]), o.fault_word, o.fault_mask);
+                    hbm_probe_r128<kRegThreads, kRegUnroll><<<(int)g->sms * kRegCtasPerSm, kRegThreads, 0, g->stream>>>(
+                        dbuf[0], dbuf[1], n_vec, s, s ^ next, ctl, out_d, seq);
+                    if (poke && f == B2DP_HL_D2H)
+                        hbm_poke<<<1, 1, 0, g->stream>>>(reinterpret_cast<uint32_t*>(dbuf[1]), o.fault_word, o.fault_mask);
+                    HL_TRY(cudaGetLastError());
+                    HL_TRY(cudaEventRecord(ev[2], g->stream));
+                    HL_TRY(cudaMemcpyAsync(host[1], dbuf[1], bytes, cudaMemcpyDeviceToHost, g->stream));
+                    HL_TRY(cudaEventRecord(ev[3], g->stream));
+                    if (!wait(ev[3], "host-link copies")) goto done;
+                    HL_TRY(cudaEventElapsedTime(&ms, f == B2DP_HL_H2D ? ev[0] : ev[2], f == B2DP_HL_H2D ? ev[1] : ev[3]));
+                } else {
+                    HL_TRY(cudaEventRecord(ev[0], g->stream));
+                    hostlink_sm<kHlThreads, kHlUnroll><<<grid, kHlThreads, 0, g->stream>>>(
+                        hdev[0], hdev[1], n_vec, s, s ^ next, poke ? o.fault_word : 0ull, poke ? o.fault_mask : 0u, ctl,
+                        out_d, seq, rec_d);
+                    HL_TRY(cudaGetLastError());
+                    HL_TRY(cudaEventRecord(ev[1], g->stream));
+                    if (!wait(ev[1], "hostlink_sm")) goto done;
+                    HL_TRY(cudaEventElapsedTime(&ms, ev[0], ev[1]));
+                }
+                ms_sum += ms;
+                std::atomic_thread_fence(std::memory_order_acquire);
+                ProbeOut po;
+                memcpy(&po, (const void*)out_h, sizeof po);  // published by the kernel's last CTA; the stream is done
+                if (po.seq != seq) ev_.seq_ok = false;
+                if (po.checksum != expected_checksum_from_counts(bc, n_words, s)) ev_.checksums_ok = false;
+                unsigned long long first = po.mismatches ? po.first_bad : ~0ull;
+                unsigned long long bad = po.mismatches + hl_check(hd, n_words, next, &first);
+                if (f == B2DP_HL_SM) {
+                    for (int c = 0; c < grid; ++c) {
+                        const HlRecord& rc = rec_h[c];
+                        if (rc.seq != seq) { ev_.seq_ok = false; continue; }
+                        if (rc.smid >= (uint32_t)kCtMaxSmId) continue;
+                        seen[rc.smid] = 1;
+                        if (rc.mismatches) r->bad_sm_mask[rc.smid / 64] |= 1ull << (rc.smid % 64);
+                    }
+                }
+                r->mismatches[f] += bad;
+                r->first_bad_word[f] = std::min<uint64_t>(r->first_bad_word[f], first);
+                ++r->rounds[f];
+                s = next;
+            }
+            r->ms[f] = (float)ms_sum;
+            const double moved = (f == B2DP_HL_SM ? 2.0 : 1.0) * (double)bytes * (double)r->rounds[f];
+            if (ms_sum > 0) r->gbs[f] = (float)(moved / ms_sum * 1e-6);
+        }
+        for (int sm = 0; sm < kCtMaxSmId; ++sm) r->sms_covered += seen[sm];
+    }
+done:
+#undef HL_TRY
+    release();
+    unsigned replays1 = replays0;
+    if (have_replays && be->nvml.pcie_replays(g->nvh, &replays1) == 0 && replays1 > replays0)
+        r->replays = replays1 - replays0;
+    if (!sampled || !have_replays) r->flags |= B2DP_HL_NO_NVML;
+    if (r->replays) r->flags |= B2DP_HL_REPLAYS;
+    if (r->link_width > 0 && r->max_link_width > 0 && r->link_width < r->max_link_width) r->flags |= B2DP_HL_LINK_NARROW;
+    if (r->link_gen > 0 && r->max_link_gen > 0 && r->link_gen < r->max_link_gen) r->flags |= B2DP_HL_LINK_SLOW;
+    r->link_gbs = (float)hl_link_gbs(r->link_gen, r->link_width);
+    if (ce != cudaSuccess) {
+        cudaGetLastError();
+        r->err = B2DP_E_CUDA;
+        r->healthy = 0;
+        *err = cuda_err(where, ce) + " on " + g->dev.id;
+    } else if (timed_out) {
+        r->err = B2DP_E_TIMEOUT;
+        r->healthy = 0;
+    } else {
+        for (int f = 0; f < kHlFormats; ++f) {
+            ev_.rounds[f] = r->rounds[f];
+            ev_.mismatches[f] = r->mismatches[f];
+        }
+        r->healthy = hl_healthy(ev_) ? 1 : 0;
+    }
+}
+
+static int cuda_hostlink_test(CudaBackend* be, int device, const b2dp_hostlink_opts* opts,
+                              std::vector<b2dp_hostlink_result>& out, std::string& err) {
+    if (be->units) {
+        err = "the host-link self-test runs in-process only (not with probe=helpers / probe=off / MIG)";
+        return B2DP_E_UNSUPPORTED;
+    }
+    if (device < -1 || device >= (int)be->gpus.size()) { err = "device index out of range"; return B2DP_E_INVAL; }
+    const b2dp_hostlink_opts o = opts ? *opts : b2dp_hostlink_opts{};
+    const unsigned long long bytes = hl_buffer_bytes(o.bytes);
+    if (!bytes) { err = "bytes must be a multiple of 16 and at most 1 GiB"; return B2DP_E_INVAL; }
+    const uint32_t duration_ms = o.duration_ms ? o.duration_ms : kHostlinkDefaultMs;
+    const uint32_t timeout_ms = o.timeout_ms ? o.timeout_ms : 10000u + 3u * duration_ms;
+    bool latched = false;
+    {
+        std::lock_guard<std::mutex> pl(be->probe_mu);  // a heartbeat waits for a running self-test
+        const uint32_t seed = (uint32_t)std::chrono::steady_clock::now().time_since_epoch().count() * kPatternMul;
+        std::vector<size_t> sel;
+        for (size_t i = 0; i < be->gpus.size(); ++i) if (device < 0 || (int)i == device) sel.push_back(i);
+        out.assign(sel.size(), b2dp_hostlink_result{});
+        std::vector<std::string> errs(sel.size());
+        std::vector<std::shared_ptr<Completion>> cs(sel.size());
+        for (size_t k = 0; k < sel.size(); ++k) {
+            Gpu* g = be->gpus[sel[k]].get();
+            b2dp_hostlink_result* r = &out[k];
+            r->device = (int32_t)sel[k];
+            r->seed = seed ^ ((uint32_t)sel[k] << 16);
+            r->sm_count = (int32_t)g->sms;
+            r->host_numa_node = -1;
+            for (auto& w : r->first_bad_word) w = ~0ull;
+            if (g->broken) { r->err = B2DP_E_CUDA; errs[k] = g->broken_reason + " on " + g->dev.id; continue; }
+            if (!(o.flags & B2DP_HL_EVEN_IF_BUSY) && used_by_another_process(be, g)) {
+                r->flags |= B2DP_HL_SKIPPED_BUSY;
+                r->healthy = g->last_healthy;
+                continue;
+            }
+            std::string* e = &errs[k];
+            cs[k] = post(g, [be, g, o, bytes, duration_ms, timeout_ms, r, e] {
+                hostlink_one(be, g, o, bytes, duration_ms, timeout_ms, r, e);
+            });
+        }
+        for (size_t k = 0; k < sel.size(); ++k) {
+            if (cs[k]) cs[k]->wait();  // no deadline here: the buffers must be released before the call returns
+            if (!errs[k].empty()) err = errs[k];
+            if (!cs[k]) continue;       // skipped (busy) or never set up: nothing ran, nothing is latched
+            Gpu* g = be->gpus[sel[k]].get();
+            const b2dp_hostlink_result& r = out[k];
+            if (!r.healthy) { g->hostlink_fault.store(true); latched = true; }
+            logf(r.healthy ? 0 : 2, "%s host-link test: %s, %llu MiB buffers on NUMA node %d, rounds %llu/%llu/%llu, "
+                 "mismatches h2d/d2h/sm %llu/%llu/%llu, %.2f/%.2f/%.2f GB/s, SMs %d/%d, PCIe gen %d/%d x%d/%d "
+                 "(%.1f GB/s), replays %llu, flags 0x%x%s", g->dev.id.c_str(),
+                 r.healthy ? "Healthy" : "Unhealthy (latched)", bytes >> 20, r.host_numa_node,
+                 (unsigned long long)r.rounds[0], (unsigned long long)r.rounds[1], (unsigned long long)r.rounds[2],
+                 (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
+                 (unsigned long long)r.mismatches[2], r.gbs[0], r.gbs[1], r.gbs[2], r.sms_covered, r.sm_count,
+                 r.link_gen, r.max_link_gen, r.link_width, r.max_link_width, r.link_gbs,
+                 (unsigned long long)r.replays, r.flags, r.err == B2DP_E_TIMEOUT ? ", timed out" : "");
+        }
+    }
+    // like the Xid latch: running ListAndWatch loops send a heartbeat now (no backend lock is held while they do)
+    if (latched) be->fire_health_event();
+    return B2DP_OK;
+}
+
 static bool cuda_diag_latched(CudaBackend* be) {
     for (auto& g : be->gpus)
-        if (g->memtest_fault.load() || g->compute_fault.load()) return true;
+        if (g->memtest_fault.load() || g->compute_fault.load() || g->hostlink_fault.load()) return true;
     return false;
 }
 
 // registered when the library is loaded, before any entry point can run (internal.hpp DiagHooks)
 [[maybe_unused]] static const bool kDiagRegistered = [] {
     diag_hooks() = DiagHooks{cuda_memtest, cuda_compute_test, cuda_fp_test, cuda_diag_latched, cuda_sfu_test,
-                             cuda_smem_test, cuda_regfile_test, cuda_int_test, cuda_l2_test};
+                             cuda_smem_test, cuda_regfile_test, cuda_int_test, cuda_l2_test, cuda_hostlink_test};
     return true;
 }();
 

@@ -66,6 +66,8 @@ struct Flags {
                                                      // register-file test), for compute_test_ms per format
     int l2_test_at_start = 0;                        // likewise for the L2 self-test (after the integer test), for
                                                      // compute_test_ms per format
+    int hostlink_test_at_start = 0;                  // likewise for the host-link self-test (after the L2 test), for
+                                                     // compute_test_ms per format
     bool version = false;
     bool labels_mode = false, reconcile = false, patch = false;
     std::string labels;                              // csv of generator names, or "all"
@@ -111,6 +113,7 @@ bool parse_flags(int argc, char** argv, Flags& f, std::string& err) {
         else if (name == "regfile_test_at_start") f.regfile_test_at_start = atoi(val.c_str());
         else if (name == "int_test_at_start") f.int_test_at_start = atoi(val.c_str());
         else if (name == "l2_test_at_start") f.l2_test_at_start = atoi(val.c_str());
+        else if (name == "hostlink_test_at_start") f.hostlink_test_at_start = atoi(val.c_str());
         else if (name == "labels") { f.labels_mode = true; f.labels = val; }
         else { err = "flag provided but not defined: -" + name; return false; }
     }
@@ -711,6 +714,32 @@ void run_l2_test(b2dp_ctx* ctx, const Flags& fl) {
     }
 }
 
+// -hostlink_test_at_start=1: likewise for the host-link self-test (the probe's pattern between host memory and the GPU,
+// by copy engine and by the SMs' own loads and stores), after the L2 test, for -compute_test_ms per format.
+void run_hostlink_test(b2dp_ctx* ctx, const Flags& fl) {
+    b2dp_hostlink_opts o{};
+    o.duration_ms = fl.compute_test_ms;
+    if (fl.hostlink_test_at_start >= 2) o.flags |= B2DP_HL_EVEN_IF_BUSY;
+    b2dp_hostlink_result res[64];
+    int n = 0;
+    const int rc = b2dp_hostlink_test(ctx, -1, &o, res, 64, &n);
+    if (rc != B2DP_OK) {
+        logf("host-link test at start not run: %s (%s)", b2dp_strerror(rc), b2dp_last_error(ctx));
+        return;
+    }
+    std::vector<b2dp_device> devs(n > 0 ? n : 1);
+    int nd = 0;
+    if (b2dp_enumerate(ctx, devs.data(), (int)devs.size(), &nd) != B2DP_OK) nd = 0;
+    for (int i = 0; i < n; ++i) {
+        const b2dp_hostlink_result& r = res[i];
+        logf("host-link test %s: %s, flags 0x%x, mismatches %llu/%llu/%llu, %.2f/%.2f/%.2f GB/s h2d/d2h/sm, "
+             "PCIe gen %d x%d, replays %llu", r.device < nd ? devs[r.device].id : "?",
+             r.healthy ? "Healthy" : "Unhealthy", r.flags, (unsigned long long)r.mismatches[0],
+             (unsigned long long)r.mismatches[1], (unsigned long long)r.mismatches[2], r.gbs[0], r.gbs[1], r.gbs[2],
+             r.link_gen, r.link_width, (unsigned long long)r.replays);
+    }
+}
+
 }  // namespace
 
 int main(int argc, char** argv) {
@@ -749,6 +778,7 @@ int main(int argc, char** argv) {
     if (fl.regfile_test_at_start) run_regfile_test(ctx, fl);
     if (fl.int_test_at_start) run_int_test(ctx, fl);
     if (fl.l2_test_at_start) run_l2_test(ctx, fl);
+    if (fl.hostlink_test_at_start) run_hostlink_test(ctx, fl);
     char names[64][64];
     int n_res = 0;
     rc = b2dp_resource_list(ctx, fl.strategy.c_str(), names, 64, &n_res);  // main.go:141-146

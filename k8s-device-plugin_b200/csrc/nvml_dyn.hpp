@@ -63,6 +63,12 @@ struct Nvml {
     int (*attributes)(void*, NvmlDeviceAttributes*) = nullptr;         // nvmlDeviceGetAttributes_v2
     int (*nvlink_state)(void*, unsigned, unsigned*) = nullptr;         // nvmlDeviceGetNvLinkState
     int (*p2p_status)(void*, void*, int, int*) = nullptr;              // nvmlDeviceGetP2PStatus
+    // PCIe link (the host-link self-test reports these; none of them is judged)
+    int (*pcie_gen)(void*, unsigned*) = nullptr;                       // nvmlDeviceGetCurrPcieLinkGeneration
+    int (*pcie_width)(void*, unsigned*) = nullptr;                     // nvmlDeviceGetCurrPcieLinkWidth
+    int (*pcie_max_gen)(void*, unsigned*) = nullptr;                   // nvmlDeviceGetMaxPcieLinkGeneration
+    int (*pcie_max_width)(void*, unsigned*) = nullptr;                 // nvmlDeviceGetMaxPcieLinkWidth
+    int (*pcie_replays)(void*, unsigned*) = nullptr;                   // nvmlDeviceGetPcieReplayCounter
     bool ok = false;
 
     ~Nvml() {
@@ -110,6 +116,11 @@ struct Nvml {
         sym(attributes, "nvmlDeviceGetAttributes_v2");
         sym(nvlink_state, "nvmlDeviceGetNvLinkState");
         sym(p2p_status, "nvmlDeviceGetP2PStatus");
+        sym(pcie_gen, "nvmlDeviceGetCurrPcieLinkGeneration");
+        sym(pcie_width, "nvmlDeviceGetCurrPcieLinkWidth");
+        sym(pcie_max_gen, "nvmlDeviceGetMaxPcieLinkGeneration");
+        sym(pcie_max_width, "nvmlDeviceGetMaxPcieLinkWidth");
+        sym(pcie_replays, "nvmlDeviceGetPcieReplayCounter");
         ok = init && init() == 0;
     }
 };

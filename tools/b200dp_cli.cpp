@@ -10,6 +10,7 @@
 //                            | labels <csv> | alloc <size> | p2p | memtest [max_bytes] | compute_test [duration_ms]
 //                            | fp_test [duration_ms] | sfu_test [duration_ms] | smem_test [duration_ms]
 //                            | regfile_test [duration_ms] | int_test [duration_ms] | l2_test [duration_ms]
+//                            | hostlink_test [duration_ms]
 #include <algorithm>
 #include <chrono>
 #include <ctime>
@@ -299,6 +300,29 @@ int main(int argc, char** argv) {
                    r.nsmid, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
                    (unsigned long long)r.mismatches[2], r.first_bad_sm, r.first_bad_format, r.first_bad_tile, r.ms[0],
                    r.ms[1], r.ms[2], r.tflops[0], r.tflops[1], r.tflops[2]);
+            bad += !r.healthy;
+        }
+        b2dp_close(ctx);
+        return bad ? 1 : 0;
+    } else if (cmd == "hostlink_test") {  // one line per device; exit status 1 if any device is Unhealthy
+        b2dp_hostlink_opts ho{};
+        ho.duration_ms = argc > 3 ? (uint32_t)strtoul(argv[3], nullptr, 0) : 0;
+        std::vector<b2dp_hostlink_result> res(n ? n : 1);
+        int m = 0;
+        if ((rc = b2dp_hostlink_test(ctx, -1, &ho, res.data(), (int)res.size(), &m)) != B2DP_OK)
+            return die(ctx, "b2dp_hostlink_test", rc);
+        int bad = 0;
+        for (int i = 0; i < m; ++i) {
+            const b2dp_hostlink_result& r = res[i];
+            printf("%s %s err=%d flags=0x%x numa=%d sms=%d/%d rounds=%llu,%llu,%llu mismatches=%llu,%llu,%llu "
+                   "ms=%.1f,%.1f,%.1f gbs_h2d=%.2f gbs_d2h=%.2f gbs_sm=%.2f link=gen%d/%d x%d/%d link_gbs=%.1f "
+                   "replays=%llu\n",
+                   devs[r.device].id, r.healthy ? "Healthy" : "Unhealthy", r.err, r.flags, r.host_numa_node,
+                   r.sms_covered, r.sm_count, (unsigned long long)r.rounds[0], (unsigned long long)r.rounds[1],
+                   (unsigned long long)r.rounds[2], (unsigned long long)r.mismatches[0],
+                   (unsigned long long)r.mismatches[1], (unsigned long long)r.mismatches[2], r.ms[0], r.ms[1], r.ms[2],
+                   r.gbs[0], r.gbs[1], r.gbs[2], r.link_gen, r.max_link_gen, r.link_width, r.max_link_width,
+                   r.link_gbs, (unsigned long long)r.replays);
             bad += !r.healthy;
         }
         b2dp_close(ctx);
