@@ -270,10 +270,11 @@ typedef struct b2dp_probe_result {
                                       last b2dp_probe_reset) => Unhealthy, sticky */
 #define B2DP_RES_MEMTEST 0x200u    /* a b2dp_memtest of this device failed or timed out since open (or the last
                                       b2dp_probe_reset) => Unhealthy, sticky */
-#define B2DP_RES_COMPUTE 0x400u    /* a compute, FP, SFU, shared-memory, register-file, integer or L2 self-test
-                                      (b2dp_compute_test, b2dp_fp_test, b2dp_sfu_test, b2dp_smem_test,
-                                      b2dp_regfile_test, b2dp_int_test, b2dp_l2_test) of this device failed or timed
-                                      out since open (or the last b2dp_probe_reset) => Unhealthy, sticky */
+#define B2DP_RES_COMPUTE 0x400u    /* a compute, FP, SFU, shared-memory, register-file, integer, L2 or half-precision
+                                      self-test (b2dp_compute_test, b2dp_fp_test, b2dp_sfu_test, b2dp_smem_test,
+                                      b2dp_regfile_test, b2dp_int_test, b2dp_l2_test, b2dp_half_test) of this device
+                                      failed or timed out since open (or the last b2dp_probe_reset) => Unhealthy,
+                                      sticky */
 #define B2DP_RES_HOSTLINK 0x800u   /* a b2dp_hostlink_test of this device failed or timed out since open (or the last
                                       b2dp_probe_reset) => Unhealthy, sticky */
 
@@ -287,8 +288,8 @@ B2DP_API int b2dp_probe_health(b2dp_ctx *ctx, const b2dp_probe_opts *opts, b2dp_
  * event numbered `mask` for `device` (seen by contexts opened with xid=1).  The reference has no equivalent. */
 B2DP_API int b2dp_probe_inject_fault(b2dp_ctx *ctx, int device, uint64_t word_index, uint32_t mask);
 /* Re-fill the probe buffers of `device` (-1 = all) with a clean pattern; also clears a latched Xid, a latched memtest
- * failure, a latched compute-, FP-, SFU-, shared-memory-, register-file-, integer- or L2-test failure and a latched
- * host-link-test failure. */
+ * failure, a latched compute-, FP-, SFU-, shared-memory-, register-file-, integer-, L2- or half-precision-test failure
+ * and a latched host-link-test failure. */
 B2DP_API int b2dp_probe_reset(b2dp_ctx *ctx, int device);
 /* Set the bandwidth ceiling (gbs_ref) of `device` (-1 = all) the fractional floor refers to, e.g. to the site's measured
  * HBM peak; gbs_ref <= 0 restores the device's own calibration.  Also how tests move a device across the 0.8 line. */
@@ -543,6 +544,28 @@ B2DP_API int b2dp_int_test(b2dp_ctx *ctx, int device, const b2dp_compute_test_op
  * in-process probe on a device with cooperative launch only; B2DP_E_UNSUPPORTED otherwise. */
 B2DP_API int b2dp_l2_test(b2dp_ctx *ctx, int device, const b2dp_compute_test_opts *opts,
                           b2dp_compute_test_result *out, int cap, int *n);
+
+/* ---- on-demand half-precision and conversion self-test (same opts, result and latch as the tensor-core self-test) ---- */
+#define B2DP_HP_F16 0              /* b2dp_half_test's format index: f16x2 fma / add / sub / mul / min / max */
+#define B2DP_HP_BF16 1             /* bf16x2 fma / add / sub / mul / min / max */
+#define B2DP_HP_CVT 2              /* the type converters: F2FP, F2F, F2I, I2F / I2FP, FRND */
+
+/* An on-demand check of every SM's 16-bit floating-point pipes and type converters on `device` (-1 = every GPU,
+ * concurrently on their workers): evidence behind the per-GPU verdict the exporter round trip supplies in the
+ * reference (exporter/health.go:42-82), merged the same way (exporter/health.go:86-106) through the sticky
+ * B2DP_RES_COMPUTE bit.  half_selftest.cuh fills every SM with CTAs of 128 threads; every thread runs each op of the
+ * format, as inline PTX, on 12 / 12 / 9 operand sets that hold every crafted class (ties, cancellation, subnormals,
+ * overflow, signed zeros, a sticky-bit-only round-up, a double-rounding trap, saturation and NaN / infinity where the
+ * ISA defines the result) next to random values: fma.rn / .relu / .sat / .ftz, add, sub, mul, min, max, min.NaN,
+ * max.NaN and min.xorsign.abs on f16x2 (B2DP_HP_F16); fma.rn / .relu, add, sub, mul, min, max, min.NaN and max.NaN on
+ * bf16x2 (B2DP_HP_BF16); f32 to f16x2 / bf16x2 / e4m3x2 / e5m2x2 / tf32 / f16 / bf16, f16x2 to e4m3x2 / e5m2x2 and back,
+ * float to s32 / u32 / s64 and s32 / u64 / s64 to float in every rounding mode, f64 to f32 and round-to-integer
+ * (B2DP_HP_CVT).  All of it is IEEE 754 or PTX-defined arithmetic, so the host computes every result word exactly, with
+ * one rounding; every thread's fold of its result words must equal the host's check value.  tflops[] is T result
+ * words/s.  Verdict, latching, the probe lock, the busy skip, the deadline and the release of every allocation are
+ * exactly b2dp_compute_test's.  cuda: backend with the in-process probe only; B2DP_E_UNSUPPORTED otherwise. */
+B2DP_API int b2dp_half_test(b2dp_ctx *ctx, int device, const b2dp_compute_test_opts *opts,
+                            b2dp_compute_test_result *out, int cap, int *n);
 
 /* ---- on-demand host-link self-test (feeds the same per-GPU verdict as the probe) ---- */
 typedef struct b2dp_hostlink_opts {

@@ -41,6 +41,7 @@
 #include "nvml_dyn.hpp"
 #include "pattern_math.hpp"
 #include "fp_selftest.cuh"
+#include "half_selftest.cuh"
 #include "int_selftest.cuh"
 #include "l2_selftest.cuh"
 #include "rf_selftest.cuh"
@@ -1590,13 +1591,14 @@ static int cuda_memtest(CudaBackend* be, int device, const b2dp_memtest_opts* op
 }
 
 // ---- on-demand compute self-tests (b2dp_compute_test, b2dp_fp_test, b2dp_sfu_test, b2dp_smem_test,
-// b2dp_regfile_test, b2dp_int_test, b2dp_l2_test) ---------------------------------------------------------------------
+// b2dp_regfile_test, b2dp_int_test, b2dp_l2_test, b2dp_half_test) ---------------------------------------------------
 // One launch per format on one GPU, on that GPU's worker: tc_selftest.cuh (tensor cores: BF16, FP8, INT8),
 // fp_selftest.cuh (FP32 FMA, FP64 FMA, FP64 tensor cores), sfu_selftest.cuh (the special-function unit),
 // smem_selftest.cuh (shared memory and the SM-to-SM DSMEM path), rf_selftest.cuh (the register file), int_selftest.cuh
-// (the integer pipes and the warp-exchange network) or l2_selftest.cuh (the L2 and its atomic units).  The host builds
+// (the integer pipes and the warp-exchange network), l2_selftest.cuh (the L2 and its atomic units) or half_selftest.cuh
+// (the 16-bit pipes and the type converters).  The host builds
 // every operand table and every comparison value itself (compute_test_math.hpp, fp_test_math.hpp, smem_test_math.hpp,
-// rf_test_math.hpp, int_test_math.hpp): a health test must not ask the device under test for its own reference values.  The SFU test departs from that rule, because no
+// rf_test_math.hpp, int_test_math.hpp, half_test_math.hpp): a health test must not ask the device under test for its own reference values.  The SFU test departs from that rule, because no
 // bit-level model of MUFU is published: its reference step (sfu_reference) runs one CTA on every SM, takes each result
 // word's majority over the SMs, names every SM that disagrees, and bounds the majority against the exact function on
 // the host; no SM is ever judged against its own output.  The tests share this driver -- grid sizing, records, tally,
@@ -1909,6 +1911,22 @@ static cudaError_t l2_scratch(Gpu* g, int fmt, int grid, size_t* bytes, uint32_t
     return cudaSuccess;
 }
 
+// ---- the half-precision and conversion test's suite ----
+static const CtKernel kHpKernels[kHpFormats] = {half_selftest<HP_F16, false>, half_selftest<HP_BF16, false>,
+                                                half_selftest<HP_CVT, false>};
+static const uint32_t kHpSmem[kHpFormats] = {0, 0, 0};
+static const uint32_t kHpTableBytes[kHpFormats] = {hp_table_bytes(HP_F16), hp_table_bytes(HP_BF16),
+                                                   hp_table_bytes(HP_CVT)};
+static void hp_suite_tile(uint32_t seed, int fmt, int tile, uint8_t* table, uint32_t* check) {
+    hp_build_tile(seed, fmt, tile, reinterpret_cast<uint32_t*>(table), check);
+}
+// tflops[] = 2 x this x comparisons / ms: T result words/s
+static double hp_suite_half_results(int fmt) { return 0.5 * hp_ops_per_tile(fmt); }
+
+static const DiagSuite kHalfSuite = {"half-precision test", "half_selftest", "f16/bf16/cvt", kHpKernels, kHpSmem,
+                                     kHpTableBytes, hp_suite_tile, hp_suite_half_results, false, nullptr,
+                                     "%.2f/%.2f/%.2f T results/s", nullptr, false, "half-precision self-test"};
+
 static const DiagSuite kL2Suite = {"L2 test", "l2_selftest", "word/byte/atom", kL2Kernels, kL2Smem, kL2TableBytes,
                                    l2_suite_tile, nullptr, false, nullptr, "%.2f/%.2f/%.2f TB/s, TB/s, G ops/s",
                                    l2_size_grid, true, "L2 self-test", l2_scratch, true};
@@ -2205,6 +2223,11 @@ static int cuda_l2_test(CudaBackend* be, int device, const b2dp_compute_test_opt
     return cuda_diag_test(kL2Suite, be, device, opts, out, err);
 }
 
+static int cuda_half_test(CudaBackend* be, int device, const b2dp_compute_test_opts* opts,
+                          std::vector<b2dp_compute_test_result>& out, std::string& err) {
+    return cuda_diag_test(kHalfSuite, be, device, opts, out, err);
+}
+
 // ---- on-demand host-link self-test (b2dp_hostlink_test) ---------------------------------------------------------------
 // Host memory -> PCIe -> copy engines / SMs -> HBM and back, on the GPU's worker.  Two host buffers (Hs, the source the
 // host writes, and Hd, the destination the host checks) are mmap'd, bound to the GPU's NUMA node before their first
@@ -2496,7 +2519,8 @@ static bool cuda_diag_latched(CudaBackend* be) {
 // registered when the library is loaded, before any entry point can run (internal.hpp DiagHooks)
 [[maybe_unused]] static const bool kDiagRegistered = [] {
     diag_hooks() = DiagHooks{cuda_memtest, cuda_compute_test, cuda_fp_test, cuda_diag_latched, cuda_sfu_test,
-                             cuda_smem_test, cuda_regfile_test, cuda_int_test, cuda_l2_test, cuda_hostlink_test};
+                             cuda_smem_test, cuda_regfile_test, cuda_int_test, cuda_l2_test, cuda_hostlink_test,
+                             cuda_half_test};
     return true;
 }();
 
