@@ -270,9 +270,9 @@ typedef struct b2dp_probe_result {
                                       last b2dp_probe_reset) => Unhealthy, sticky */
 #define B2DP_RES_MEMTEST 0x200u    /* a b2dp_memtest of this device failed or timed out since open (or the last
                                       b2dp_probe_reset) => Unhealthy, sticky */
-#define B2DP_RES_COMPUTE 0x400u    /* a compute, FP, SFU, shared-memory, register-file, integer, L2 or half-precision
-                                      self-test (b2dp_compute_test, b2dp_fp_test, b2dp_sfu_test, b2dp_smem_test,
-                                      b2dp_regfile_test, b2dp_int_test, b2dp_l2_test, b2dp_half_test) of this device
+#define B2DP_RES_COMPUTE 0x400u    /* a compute, FP, SFU, shared-memory, register-file, integer, L2, half-precision or
+                                      synchronization self-test (b2dp_compute_test, b2dp_fp_test, b2dp_sfu_test, b2dp_smem_test,
+                                      b2dp_regfile_test, b2dp_int_test, b2dp_l2_test, b2dp_half_test, b2dp_sync_test) of this device
                                       failed or timed out since open (or the last b2dp_probe_reset) => Unhealthy,
                                       sticky */
 #define B2DP_RES_HOSTLINK 0x800u   /* a b2dp_hostlink_test of this device failed or timed out since open (or the last
@@ -565,6 +565,27 @@ B2DP_API int b2dp_l2_test(b2dp_ctx *ctx, int device, const b2dp_compute_test_opt
  * words/s.  Verdict, latching, the probe lock, the busy skip, the deadline and the release of every allocation are
  * exactly b2dp_compute_test's.  cuda: backend with the in-process probe only; B2DP_E_UNSUPPORTED otherwise. */
 B2DP_API int b2dp_half_test(b2dp_ctx *ctx, int device, const b2dp_compute_test_opts *opts,
+                            b2dp_compute_test_result *out, int cap, int *n);
+
+/* ---- on-demand synchronization self-test (same opts, result and latch as the tensor-core self-test) ---- */
+#define B2DP_SY_ATOM 0             /* b2dp_sync_test's format index: the shared-memory atomic unit */
+#define B2DP_SY_BAR 1              /* named barriers, bar.red and the mbarriers */
+#define B2DP_SY_WARP 2             /* shfl / vote / redux / match / elect / __syncwarp in diverged warps */
+
+/* An on-demand check of every SM's synchronization hardware on `device` (-1 = every GPU, concurrently on their
+ * workers): evidence behind the per-GPU verdict the exporter round trip supplies in the reference
+ * (exporter/health.go:42-82), merged the same way (exporter/health.go:86-106) through the sticky B2DP_RES_COMPUTE bit.
+ * sync_selftest.cuh fills every SM with CTAs of 128 threads.  B2DP_SY_ATOM runs atom.shared add / inc / dec / exch /
+ * cas / and / or / xor / min / max on 32 and 64 bits, red.shared and float adds (f32, f64, f16x2, bf16x2) on a per-lane
+ * plane, a same-bank plane and a hot word; B2DP_SY_BAR runs bar.arrive / bar.sync on ids 1-15 at 64, 96 and 128 threads,
+ * bar.red.popc / and / or, and an mbarrier through arrive counts, noComplete, arrive_drop, expect_tx and complete_tx;
+ * B2DP_SY_WARP runs shfl / vote / redux / match / elect.sync, activemask and __syncwarp inside diverged groups of three
+ * nested partitions.  Every expected value follows from the PTX ISA, so the host computes every result word; every
+ * thread's fold of its result words must equal the host's check value.  Every wait is bounded by the deadline plus a
+ * grace period.  tflops[] is G atomic ops/s, G barrier ops/s and T result words/s.  Verdict, latching, the probe lock,
+ * the busy skip, the deadline and the release of every allocation are exactly b2dp_compute_test's.  cuda: backend with
+ * the in-process probe only; B2DP_E_UNSUPPORTED otherwise. */
+B2DP_API int b2dp_sync_test(b2dp_ctx *ctx, int device, const b2dp_compute_test_opts *opts,
                             b2dp_compute_test_result *out, int cap, int *n);
 
 /* ---- on-demand host-link self-test (feeds the same per-GPU verdict as the probe) ---- */

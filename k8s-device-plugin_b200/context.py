@@ -65,7 +65,7 @@ class ComputeTestResult:
     tflops: List[float]            # 2 M N K x result tiles compared / ms (TOPS for INT8; fp_test: 2 x FMAs / ms;
                                    # sfu_test: MUFU results / ms, in T results/s; smem_test, regfile_test: TB/s;
                                    # int_test, half_test: result words / ms, in T results/s; l2_test: TB/s, TB/s,
-                                   # G ops/s)
+                                   # G ops/s; sync_test: G ops/s, G ops/s, T results/s)
 
     def bad_sms(self) -> List[int]:
         return [s for s in range(256) if (self.bad_sm_mask[s // 64] >> (s % 64)) & 1]
@@ -360,6 +360,22 @@ class Context:
         opts = N.ComputeTestOpts(duration_ms, timeout_ms, N.CT_EVEN_IF_BUSY if even_if_busy else 0, fault_sm, fault_mask, 0)
         rc, arr, n = N.grow_call(lambda cap: (N.ComputeTestResult * cap)(),
                                  lambda a, cap, pn: N.lib.b2dp_half_test(self._h, device, C.byref(opts), a, cap, pn))
+        N.check(rc, self._h)
+        return [ComputeTestResult(r.device, bool(r.healthy), r.err, r.flags, r.seed, r.sm_count, r.nsmid, r.sms_covered,
+                                  list(r.bad_sm_mask), list(r.mismatches), r.first_bad_sm, r.first_bad_format,
+                                  r.first_bad_tile, list(r.ms), list(r.tflops)) for r in arr[:n]]
+
+    def sync_test(self, device: int = -1, duration_ms: int = 0, timeout_ms: int = 0, even_if_busy: bool = False,
+                  fault_sm: int = -1, fault_mask: int = 0) -> List[ComputeTestResult]:
+        """On-demand synchronization self-test of `device` (-1 = every GPU, b2dp_sync_test): every SM's shared-memory
+        atomics, named barriers, bar.red, mbarriers and warp collectives under partial member masks, against results the
+        host computed from the PTX ISA, for duration_ms per format (0 = 1000).  The per-format lists are indexed by
+        SY_ATOM, SY_BAR, SY_WARP; tflops holds G atomic ops/s, G barrier ops/s and T result words/s.  A failure is
+        latched like compute_test()'s (RES_COMPUTE until probe_reset()); fault_sm / fault_mask flips bits of one result
+        word of one thread of the SM with that %smid, in the first comparison."""
+        opts = N.ComputeTestOpts(duration_ms, timeout_ms, N.CT_EVEN_IF_BUSY if even_if_busy else 0, fault_sm, fault_mask, 0)
+        rc, arr, n = N.grow_call(lambda cap: (N.ComputeTestResult * cap)(),
+                                 lambda a, cap, pn: N.lib.b2dp_sync_test(self._h, device, C.byref(opts), a, cap, pn))
         N.check(rc, self._h)
         return [ComputeTestResult(r.device, bool(r.healthy), r.err, r.flags, r.seed, r.sm_count, r.nsmid, r.sms_covered,
                                   list(r.bad_sm_mask), list(r.mismatches), r.first_bad_sm, r.first_bad_format,

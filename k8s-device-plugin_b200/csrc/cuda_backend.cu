@@ -45,6 +45,7 @@
 #include "int_selftest.cuh"
 #include "l2_selftest.cuh"
 #include "rf_selftest.cuh"
+#include "sync_selftest.cuh"
 #include "sfu_selftest.cuh"
 #include "smem_selftest.cuh"
 #include "tc_selftest.cuh"
@@ -1927,6 +1928,21 @@ static const DiagSuite kHalfSuite = {"half-precision test", "half_selftest", "f1
                                      kHpTableBytes, hp_suite_tile, hp_suite_half_results, false, nullptr,
                                      "%.2f/%.2f/%.2f T results/s", nullptr, false, "half-precision self-test"};
 
+// ---- the synchronization test's suite ----
+static const CtKernel kSyKernels[kSyFormats] = {sync_selftest<SY_ATOM, false>, sync_selftest<SY_BAR, false>,
+                                                sync_selftest<SY_WARP, false>};
+static const uint32_t kSySmem[kSyFormats] = {0, 0, 0};
+static const uint32_t kSyTableBytes[kSyFormats] = {sy_table_bytes(SY_ATOM), sy_table_bytes(SY_BAR),
+                                                   sy_table_bytes(SY_WARP)};
+static void sy_suite_tile(uint32_t seed, int fmt, int tile, uint8_t* table, uint32_t* check) {
+    sy_build_tile(seed, fmt, tile, reinterpret_cast<uint32_t*>(table), check);
+}
+
+static const DiagSuite kSyncSuite = {"sync test", "sync_selftest", "atom/bar/warp", kSyKernels, kSySmem,
+                                     kSyTableBytes, sy_suite_tile, sy_rate_half_units, false, nullptr,
+                                     "%.2f/%.2f/%.2f G atomic ops/s, G barrier ops/s, T results/s", nullptr, false,
+                                     "synchronization self-test"};
+
 static const DiagSuite kL2Suite = {"L2 test", "l2_selftest", "word/byte/atom", kL2Kernels, kL2Smem, kL2TableBytes,
                                    l2_suite_tile, nullptr, false, nullptr, "%.2f/%.2f/%.2f TB/s, TB/s, G ops/s",
                                    l2_size_grid, true, "L2 self-test", l2_scratch, true};
@@ -2228,6 +2244,11 @@ static int cuda_half_test(CudaBackend* be, int device, const b2dp_compute_test_o
     return cuda_diag_test(kHalfSuite, be, device, opts, out, err);
 }
 
+static int cuda_sync_test(CudaBackend* be, int device, const b2dp_compute_test_opts* opts,
+                          std::vector<b2dp_compute_test_result>& out, std::string& err) {
+    return cuda_diag_test(kSyncSuite, be, device, opts, out, err);
+}
+
 // ---- on-demand host-link self-test (b2dp_hostlink_test) ---------------------------------------------------------------
 // Host memory -> PCIe -> copy engines / SMs -> HBM and back, on the GPU's worker.  Two host buffers (Hs, the source the
 // host writes, and Hd, the destination the host checks) are mmap'd, bound to the GPU's NUMA node before their first
@@ -2520,7 +2541,7 @@ static bool cuda_diag_latched(CudaBackend* be) {
 [[maybe_unused]] static const bool kDiagRegistered = [] {
     diag_hooks() = DiagHooks{cuda_memtest, cuda_compute_test, cuda_fp_test, cuda_diag_latched, cuda_sfu_test,
                              cuda_smem_test, cuda_regfile_test, cuda_int_test, cuda_l2_test, cuda_hostlink_test,
-                             cuda_half_test};
+                             cuda_half_test, cuda_sync_test};
     return true;
 }();
 

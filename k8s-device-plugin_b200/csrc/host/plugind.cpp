@@ -70,6 +70,8 @@ struct Flags {
                                                      // compute_test_ms per format
     int half_test_at_start = 0;                      // likewise for the half-precision and conversion self-test (after
                                                      // the host-link test), for compute_test_ms per format
+    int sync_test_at_start = 0;                      // likewise for the synchronization self-test (after the
+                                                     // half-precision test), for compute_test_ms per format
     bool version = false;
     bool labels_mode = false, reconcile = false, patch = false;
     std::string labels;                              // csv of generator names, or "all"
@@ -116,6 +118,7 @@ bool parse_flags(int argc, char** argv, Flags& f, std::string& err) {
         else if (name == "int_test_at_start") f.int_test_at_start = atoi(val.c_str());
         else if (name == "l2_test_at_start") f.l2_test_at_start = atoi(val.c_str());
         else if (name == "half_test_at_start") f.half_test_at_start = atoi(val.c_str());
+        else if (name == "sync_test_at_start") f.sync_test_at_start = atoi(val.c_str());
         else if (name == "hostlink_test_at_start") f.hostlink_test_at_start = atoi(val.c_str());
         else if (name == "labels") { f.labels_mode = true; f.labels = val; }
         else { err = "flag provided but not defined: -" + name; return false; }
@@ -769,6 +772,32 @@ void run_half_test(b2dp_ctx* ctx, const Flags& fl) {
     }
 }
 
+// -sync_test_at_start=1: likewise for the synchronization self-test (shared-memory atomics, barriers, mbarriers and
+// warp collectives against the PTX ISA), after the half-precision test, for -compute_test_ms per format.
+void run_sync_test(b2dp_ctx* ctx, const Flags& fl) {
+    b2dp_compute_test_opts o{};
+    o.duration_ms = fl.compute_test_ms;
+    o.fault_sm = -1;
+    if (fl.sync_test_at_start >= 2) o.flags |= B2DP_CT_EVEN_IF_BUSY;
+    b2dp_compute_test_result res[64];
+    int n = 0;
+    const int rc = b2dp_sync_test(ctx, -1, &o, res, 64, &n);
+    if (rc != B2DP_OK) {
+        logf("sync test at start not run: %s (%s)", b2dp_strerror(rc), b2dp_last_error(ctx));
+        return;
+    }
+    std::vector<b2dp_device> devs(n > 0 ? n : 1);
+    int nd = 0;
+    if (b2dp_enumerate(ctx, devs.data(), (int)devs.size(), &nd) != B2DP_OK) nd = 0;
+    for (int i = 0; i < n; ++i) {
+        const b2dp_compute_test_result& r = res[i];
+        logf("sync test %s: %s, flags 0x%x, SMs %d/%d, mismatches %llu/%llu/%llu, first bad SM %d, %.2f/%.2f/%.2f "
+             "G ops/s, G ops/s, T results/s", r.device < nd ? devs[r.device].id : "?", r.healthy ? "Healthy" : "Unhealthy", r.flags,
+             r.sms_covered, r.sm_count, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
+             (unsigned long long)r.mismatches[2], r.first_bad_sm, r.tflops[0], r.tflops[1], r.tflops[2]);
+    }
+}
+
 }  // namespace
 
 int main(int argc, char** argv) {
@@ -809,6 +838,7 @@ int main(int argc, char** argv) {
     if (fl.l2_test_at_start) run_l2_test(ctx, fl);
     if (fl.hostlink_test_at_start) run_hostlink_test(ctx, fl);
     if (fl.half_test_at_start) run_half_test(ctx, fl);
+    if (fl.sync_test_at_start) run_sync_test(ctx, fl);
     char names[64][64];
     int n_res = 0;
     rc = b2dp_resource_list(ctx, fl.strategy.c_str(), names, 64, &n_res);  // main.go:141-146

@@ -146,8 +146,8 @@ void cuda_set_health_event_callback(CudaBackend*, std::function<void()> fn);
 // The on-demand diagnostics (the memory test and the compute and FP self-tests) are optional capabilities of the cuda backend:
 // a build of the library whose backend has none (the CPU-only build of ctx.cpp the sanitizer tests link against a
 // stand-in backend) simply leaves these null, and b2dp_memtest / b2dp_compute_test / b2dp_fp_test / b2dp_sfu_test /
-// b2dp_smem_test / b2dp_regfile_test / b2dp_int_test / b2dp_l2_test / b2dp_hostlink_test / b2dp_half_test then
-// return B2DP_E_UNSUPPORTED.
+// b2dp_smem_test / b2dp_regfile_test / b2dp_int_test / b2dp_l2_test / b2dp_hostlink_test / b2dp_half_test /
+// b2dp_sync_test then return B2DP_E_UNSUPPORTED.
 // cuda_backend.cu fills them in during static initialisation.
 struct DiagHooks {
     // b2dp_memtest on `device` (-1 = all); B2DP_E_UNSUPPORTED without the in-process probe
@@ -183,6 +183,9 @@ struct DiagHooks {
                          std::vector<b2dp_hostlink_result>& out, std::string& err) = nullptr;
     // b2dp_half_test on `device` (-1 = all); B2DP_E_UNSUPPORTED without the in-process probe
     int (*half_test)(CudaBackend*, int device, const b2dp_compute_test_opts* opts,
+                     std::vector<b2dp_compute_test_result>& out, std::string& err) = nullptr;
+    // b2dp_sync_test on `device` (-1 = all); B2DP_E_UNSUPPORTED without the in-process probe
+    int (*sync_test)(CudaBackend*, int device, const b2dp_compute_test_opts* opts,
                      std::vector<b2dp_compute_test_result>& out, std::string& err) = nullptr;
 };
 DiagHooks& diag_hooks();  // ctx.cpp
