@@ -270,9 +270,10 @@ typedef struct b2dp_probe_result {
                                       last b2dp_probe_reset) => Unhealthy, sticky */
 #define B2DP_RES_MEMTEST 0x200u    /* a b2dp_memtest of this device failed or timed out since open (or the last
                                       b2dp_probe_reset) => Unhealthy, sticky */
-#define B2DP_RES_COMPUTE 0x400u    /* a compute, FP, SFU, shared-memory, register-file, integer, L2, half-precision or
-                                      synchronization self-test (b2dp_compute_test, b2dp_fp_test, b2dp_sfu_test, b2dp_smem_test,
-                                      b2dp_regfile_test, b2dp_int_test, b2dp_l2_test, b2dp_half_test, b2dp_sync_test) of this device
+#define B2DP_RES_COMPUTE 0x400u    /* a compute, FP, SFU, shared-memory, register-file, integer, L2, half-precision,
+                                      synchronization or L1 self-test (b2dp_compute_test, b2dp_fp_test, b2dp_sfu_test,
+                                      b2dp_smem_test, b2dp_regfile_test, b2dp_int_test, b2dp_l2_test, b2dp_half_test,
+                                      b2dp_sync_test, b2dp_l1_test) of this device
                                       failed or timed out since open (or the last b2dp_probe_reset) => Unhealthy,
                                       sticky */
 #define B2DP_RES_HOSTLINK 0x800u   /* a b2dp_hostlink_test of this device failed or timed out since open (or the last
@@ -587,6 +588,27 @@ B2DP_API int b2dp_half_test(b2dp_ctx *ctx, int device, const b2dp_compute_test_o
  * the in-process probe only; B2DP_E_UNSUPPORTED otherwise. */
 B2DP_API int b2dp_sync_test(b2dp_ctx *ctx, int device, const b2dp_compute_test_opts *opts,
                             b2dp_compute_test_result *out, int cap, int *n);
+
+/* ---- on-demand L1 self-test (same opts, result and latch as the tensor-core self-test) ---- */
+#define B2DP_L1_DATA 0             /* b2dp_l1_test's format index: the L1 data cache, written and read back */
+#define B2DP_L1_TEX 1              /* the texture path and the read-only data path */
+#define B2DP_L1_CONST 2            /* the constant cache */
+
+/* An on-demand check of every SM's L1TEX unit and constant cache on `device` (-1 = every GPU, concurrently on their
+ * workers): evidence behind the per-GPU verdict the exporter round trip supplies in the reference
+ * (exporter/health.go:42-82), merged the same way (exporter/health.go:86-106) through the sticky B2DP_RES_COMPUTE bit.
+ * l1_selftest.cuh fills every SM with CTAs of 128 threads at a shared-memory carve-out of 0.  B2DP_L1_DATA writes each
+ * CTA's private span (128 KiB per SM over its CTAs) with st.global.v4 and reads it back three times with weak
+ * ld.global.v4 in ascending, descending and strided order, every word read by a thread other than its writer;
+ * B2DP_L1_TEX reads a 128 KiB block-linear CUDA array through texture objects (integer and float coordinates, wrap /
+ * mirror / clamp / border, tld4 gathers) and its linear copy with ld.global.nc; B2DP_L1_CONST reads a 32 KiB
+ * __constant__ bank at warp-uniform and lane-divergent indices with 32-, 64- and 128-bit loads.  The host builds every
+ * datum and computes every expected value; every thread's fold must equal the host's check value.  tflops[] is TB/s
+ * the loads deliver (B2DP_L1_DATA: and its stores).  Verdict, latching, the probe lock, the busy skip, the deadline and
+ * the release of every allocation (the CUDA array and the texture objects included) are exactly b2dp_compute_test's.
+ * cuda: backend with the in-process probe only; B2DP_E_UNSUPPORTED otherwise. */
+B2DP_API int b2dp_l1_test(b2dp_ctx *ctx, int device, const b2dp_compute_test_opts *opts,
+                          b2dp_compute_test_result *out, int cap, int *n);
 
 /* ---- on-demand host-link self-test (feeds the same per-GPU verdict as the probe) ---- */
 typedef struct b2dp_hostlink_opts {

@@ -53,6 +53,7 @@ RF_ALU, RF_LOAD, RF_HOLD = 0, 1, 2
 IT_MAD, IT_BIT, IT_WARP = 0, 1, 2
 HP_F16, HP_BF16, HP_CVT = 0, 1, 2
 SY_ATOM, SY_BAR, SY_WARP = 0, 1, 2
+L1_DATA, L1_TEX, L1_CONST = 0, 1, 2
 L2_WORD, L2_BYTE, L2_ATOM = 0, 1, 2
 CT_ECC_CORRECTED, CT_ECC, CT_NO_ECC = 0x10, 0x20, 0x40
 RES_HOSTLINK = 0x800
@@ -217,6 +218,7 @@ SIGNATURES = {
     "b2dp_hostlink_test": (_i, [_vp, _i, _P(HostlinkOpts), _P(HostlinkResult), _i, _ip]),
     "b2dp_half_test": (_i, [_vp, _i, _P(ComputeTestOpts), _P(ComputeTestResult), _i, _ip]),
     "b2dp_sync_test": (_i, [_vp, _i, _P(ComputeTestOpts), _P(ComputeTestResult), _i, _ip]),
+    "b2dp_l1_test": (_i, [_vp, _i, _P(ComputeTestOpts), _P(ComputeTestResult), _i, _ip]),
     "b2dp_probe_set_ref": (_i, [_vp, _i, C.c_float]),
     "b2dp_probe_describe": (_i, [_vp, _i, _P(ProbeInfo)]),
     "b2dp_expected_checksum": (_i, [C.c_uint64, C.c_uint32, _P(C.c_uint64)]),

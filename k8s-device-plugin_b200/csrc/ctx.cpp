@@ -681,6 +681,28 @@ extern "C" int b2dp_sync_test(b2dp_ctx* c, int device, const b2dp_compute_test_o
     return B2DP_OK;
 }
 
+extern "C" int b2dp_l1_test(b2dp_ctx* c, int device, const b2dp_compute_test_opts* opts,
+                            b2dp_compute_test_result* out, int cap, int* n) {
+    if (!c || !n || cap < 0) return B2DP_E_INVAL;
+    if (c->kind != b2dp_ctx::CUDA)
+        return fail(B2DP_E_UNSUPPORTED, "the L1 self-test needs the cuda: backend (there is no CPU fallback)");
+    // the capacity is checked before the test runs: its results cannot be produced a second time for free
+    const int count = cuda_device_count(c->cuda);
+    if (device < -1 || device >= count) return fail(B2DP_E_INVAL, "device index out of range");
+    *n = device < 0 ? count : 1;
+    if (*n > cap) return B2DP_E_NOSPC;
+    if (*n && !out) return B2DP_E_INVAL;
+    std::vector<b2dp_compute_test_result> res;
+    std::string err;
+    const DiagHooks& dh = diag_hooks();
+    if (!dh.l1_test) return fail(B2DP_E_UNSUPPORTED, "this build of the library has no L1 self-test");
+    int rc = dh.l1_test(c->cuda, device, opts, res, err);
+    if (rc != B2DP_OK) return fail(rc, err);
+    *n = (int)res.size();
+    memcpy(out, res.data(), res.size() * sizeof(b2dp_compute_test_result));
+    return B2DP_OK;
+}
+
 extern "C" int b2dp_merge_health(const char (*ids)[64], int n, int32_t default_healthy, int have_source,
                                  const char (*src_ids)[64], const int32_t* src_health, int m, int32_t* out) {
     if (n < 0 || m < 0 || (n && (!ids || !out)) || (have_source && m && (!src_ids || !src_health))) return B2DP_E_INVAL;

@@ -29,6 +29,8 @@
 #include <cstdlib>
 #include <deque>
 #include <functional>
+#include <map>
+#include <mutex>
 #include <thread>
 
 #include "gosem.hpp"
@@ -43,6 +45,7 @@
 #include "fp_selftest.cuh"
 #include "half_selftest.cuh"
 #include "int_selftest.cuh"
+#include "l1_selftest.cuh"
 #include "l2_selftest.cuh"
 #include "rf_selftest.cuh"
 #include "sync_selftest.cuh"
@@ -1592,7 +1595,7 @@ static int cuda_memtest(CudaBackend* be, int device, const b2dp_memtest_opts* op
 }
 
 // ---- on-demand compute self-tests (b2dp_compute_test, b2dp_fp_test, b2dp_sfu_test, b2dp_smem_test,
-// b2dp_regfile_test, b2dp_int_test, b2dp_l2_test, b2dp_half_test) ---------------------------------------------------
+// b2dp_regfile_test, b2dp_int_test, b2dp_l2_test, b2dp_half_test, b2dp_sync_test, b2dp_l1_test) ------------------
 // One launch per format on one GPU, on that GPU's worker: tc_selftest.cuh (tensor cores: BF16, FP8, INT8),
 // fp_selftest.cuh (FP32 FMA, FP64 FMA, FP64 tensor cores), sfu_selftest.cuh (the special-function unit),
 // smem_selftest.cuh (shared memory and the SM-to-SM DSMEM path), rf_selftest.cuh (the register file), int_selftest.cuh
@@ -1656,6 +1659,16 @@ struct DiagSuite {
     cudaError_t (*scratch)(Gpu* g, int fmt, int grid, size_t* bytes, uint32_t* header, double* macs_per_cta,
                            const char** where);
     bool cooperative;                          // launch with cudaLaunchCooperativeKernel (every CTA co-resident)
+    // Optional per-format shared-memory carve-out in percent (the L1 test's 0: the largest L1 the hardware allows;
+    // null: 100).
+    const int* carveout = nullptr;
+    // Optional host objects the kernels read (the L1 test's CUDA array, texture objects and constant bank; null: none).
+    // bind runs on the worker after the buffers exist and before the timed launches, with the call's seed and every
+    // format's scratch buffer; an error is a CUDA error of the call, named in *where, and nothing launches.  unbind runs
+    // in the release after the stream is synchronized, on every path, and destroys whatever bind made in *state.
+    cudaError_t (*bind)(Gpu* g, uint32_t seed, const DiagTables& tabs, uint32_t* const* scratch, void** state,
+                        const char** where) = nullptr;
+    void (*unbind)(void* state) = nullptr;
 };
 
 static void ct_suite_tile(uint32_t seed, int fmt, int tile, uint8_t* table, uint32_t* check) {
@@ -1912,6 +1925,90 @@ static cudaError_t l2_scratch(Gpu* g, int fmt, int grid, size_t* bytes, uint32_t
     return cudaSuccess;
 }
 
+// ---- the L1 test's suite ----
+static const CtKernel kL1Kernels[kL1Formats] = {l1_selftest<L1_DATA, false>, l1_selftest<L1_TEX, false>,
+                                                l1_selftest<L1_CONST, false>};
+static const uint32_t kL1Smem[kL1Formats] = {0, 0, 0};
+static const uint32_t kL1TableBytesAll[kL1Formats] = {l1_table_bytes(L1_DATA), l1_table_bytes(L1_TEX),
+                                                      l1_table_bytes(L1_CONST)};
+static const int kL1Carveout[kL1Formats] = {0, 0, 0};
+static void l1_suite_tile(uint32_t seed, int fmt, int tile, uint8_t* table, uint32_t* check) {
+    l1_build_tile(seed, fmt, tile, reinterpret_cast<uint32_t*>(table), check);
+}
+
+// Every resident CTA (no cooperative launch: no CTA waits for another).
+static cudaError_t l1_size_grid(Gpu* g, int fmt, int* grid, const char** where) {
+    int per_sm = 0;
+    cudaError_t ce = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kL1Kernels[fmt], kCtThreads, 0);
+    if (ce != cudaSuccess) { *where = "cudaOccupancyMaxActiveBlocksPerMultiprocessor(l1_selftest)"; return ce; }
+    *grid = (int)g->sms * (per_sm > 0 ? per_sm : 1);
+    return cudaSuccess;
+}
+
+// DATA: the header and every CTA's span of K blocks (kL1DefaultSpan per SM over the CTAs an SM holds); TEX: the header
+// and the linear copy of the image; CONST: the header.  *half is half of one CTA's bytes of one comparison, as
+// tflops[] = 2 x it x comparisons / ms: TB/s the loads deliver (DATA: and its stores).
+static cudaError_t l1_scratch(Gpu* g, int fmt, int grid, size_t* bytes, uint32_t* header, double* half,
+                              const char** where) {
+    const int per_sm = grid / (int)(g->sms ? g->sms : 1);
+    const uint32_t K = l1_span_blocks(kL1DefaultSpan, per_sm);
+    size_t data = 0;
+    if (fmt == L1_DATA) {
+        header[kL1HdrBlocks] = K;
+        data = (size_t)grid * K * kL1BlockWords;
+        logf(0, "%s L1 test: %d CTAs, span %u KiB per CTA, %.0f KiB per SM", g->dev.id.c_str(), grid,
+             K * kL1BlockBytes >> 10, (double)K * kL1BlockBytes * per_sm / 1024);
+    } else if (fmt == L1_TEX) {
+        data = (size_t)kL1Texels * 4;
+    }
+    *half = 0.5 * l1_bytes_per_comparison(fmt, K);
+    *bytes = ((size_t)kL1DataOff + data) * 4;
+    (void)where;
+    return cudaSuccess;
+}
+
+// The constant bank is one per device in the process, shared by every b2dp_ctx, whose probe locks do not serialize each
+// other: a bank lock per CUDA ordinal is held from bind to unbind, so no call reloads the bank under another's kernels.
+static std::mutex& l1_bank_mutex(int ordinal) {
+    static std::mutex guard;
+    static std::map<int, std::mutex> per_device;  // map nodes never move: the references stay valid
+    std::lock_guard<std::mutex> lk(guard);
+    return per_device[ordinal];
+}
+
+struct L1SuiteState {
+    std::unique_lock<std::mutex> bank;
+    L1Bound bound;
+};
+
+// The CUDA array, the texture objects (handles into L1_TEX's scratch header) and the constant bank, from the call's seed.
+// Refuses, before anything launches, an uploaded tile table whose indices leave their range (l1_selftest masks them all
+// the same).
+static cudaError_t l1_bind_suite(Gpu* g, uint32_t seed, const DiagTables& tabs, uint32_t* const* scratch, void** state,
+                                 const char** where) {
+    for (int f = 0; f < kL1Formats; ++f)
+        for (int tile = 0; tile < kCtTiles; ++tile)
+            if (tabs.tables[f].size() != (size_t)kCtTiles * l1_table_bytes(f) ||
+                !l1_table_ok(f, reinterpret_cast<const uint32_t*>(tabs.tables[f].data()) + tile * kL1TableWords)) {
+                *where = "l1_selftest: a tile table indexes outside its range";
+                return cudaErrorInvalidValue;
+            }
+    L1SuiteState* st = new L1SuiteState;
+    *state = st;
+    st->bank = std::unique_lock<std::mutex>(l1_bank_mutex(g->ordinal));
+    return l1_bind(seed, scratch[L1_TEX], g->stream, st->bound, where);
+}
+// Runs on the worker that ran bind, after the stream is synchronized: the bank is released last.
+static void l1_unbind_suite(void* state) {
+    L1SuiteState* st = static_cast<L1SuiteState*>(state);
+    l1_unbind(st->bound);
+    delete st;
+}
+
+static const DiagSuite kL1Suite = {"L1 test", "l1_selftest", "data/tex/const", kL1Kernels, kL1Smem, kL1TableBytesAll,
+                                   l1_suite_tile, nullptr, false, nullptr, "%.2f/%.2f/%.2f TB/s", l1_size_grid, true,
+                                   "L1 self-test", l1_scratch, false, kL1Carveout, l1_bind_suite, l1_unbind_suite};
+
 // ---- the half-precision and conversion test's suite ----
 static const CtKernel kHpKernels[kHpFormats] = {half_selftest<HP_F16, false>, half_selftest<HP_BF16, false>,
                                                 half_selftest<HP_CVT, false>};
@@ -1969,11 +2066,13 @@ static void compute_test_one(const DiagSuite& su, CudaBackend* be, Gpu* g, const
     CtRecord* rec_h = nullptr;
     CtRecord* rec_d = nullptr;
     cudaEvent_t ev[kCtFormats + 1] = {};
+    void* bound = nullptr;
     bool timed_out = false;
     cudaError_t ce = cudaSuccess;
     const char* where = "";
     auto release = [&] {  // every path ends here: nothing the test allocated outlives it
         if (g->stream) cudaStreamSynchronize(g->stream);
+        if (bound) su.unbind(bound);
         for (int f = 0; f < kCtFormats; ++f) {
             if (img[f]) cudaFree(img[f]);
             if (chk[f]) cudaFree(chk[f]);
@@ -1992,7 +2091,8 @@ static void compute_test_one(const DiagSuite& su, CudaBackend* be, Gpu* g, const
             for (int f = 0; f < kCtFormats; ++f) macs[f] = su.macs_per_tile(f);
         for (int f = 0; f < kCtFormats; ++f) {
             CT_TRY(cudaFuncSetAttribute(su.kernels[f], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)su.smem[f]));
-            CT_TRY(cudaFuncSetAttribute(su.kernels[f], cudaFuncAttributePreferredSharedMemoryCarveout, 100));
+            CT_TRY(cudaFuncSetAttribute(su.kernels[f], cudaFuncAttributePreferredSharedMemoryCarveout,
+                                        su.carveout ? su.carveout[f] : 100));
             if (su.size_grid) {
                 if ((ce = su.size_grid(g, f, &grid[f], &where)) != cudaSuccess) goto done;
             } else {
@@ -2033,6 +2133,7 @@ static void compute_test_one(const DiagSuite& su, CudaBackend* be, Gpu* g, const
                 CT_TRY(cudaMemcpy(scr[f], header, sizeof header, cudaMemcpyHostToDevice));
             }
         }
+        if (su.bind && (ce = su.bind(g, r->seed, *tabs, scr, &bound, &where)) != cudaSuccess) goto done;
         for (cudaEvent_t& e : ev) CT_TRY(cudaEventCreate(&e));
         // Device-wide counters, as the memory test reads them: a single-bit defect ECC corrects never reaches the data
         // check, and only the corrected count shows it.
@@ -2247,6 +2348,11 @@ static int cuda_half_test(CudaBackend* be, int device, const b2dp_compute_test_o
 static int cuda_sync_test(CudaBackend* be, int device, const b2dp_compute_test_opts* opts,
                           std::vector<b2dp_compute_test_result>& out, std::string& err) {
     return cuda_diag_test(kSyncSuite, be, device, opts, out, err);
+}
+
+static int cuda_l1_test(CudaBackend* be, int device, const b2dp_compute_test_opts* opts,
+                        std::vector<b2dp_compute_test_result>& out, std::string& err) {
+    return cuda_diag_test(kL1Suite, be, device, opts, out, err);
 }
 
 // ---- on-demand host-link self-test (b2dp_hostlink_test) ---------------------------------------------------------------
@@ -2541,7 +2647,7 @@ static bool cuda_diag_latched(CudaBackend* be) {
 [[maybe_unused]] static const bool kDiagRegistered = [] {
     diag_hooks() = DiagHooks{cuda_memtest, cuda_compute_test, cuda_fp_test, cuda_diag_latched, cuda_sfu_test,
                              cuda_smem_test, cuda_regfile_test, cuda_int_test, cuda_l2_test, cuda_hostlink_test,
-                             cuda_half_test, cuda_sync_test};
+                             cuda_half_test, cuda_sync_test, cuda_l1_test};
     return true;
 }();
 

@@ -72,6 +72,8 @@ struct Flags {
                                                      // the host-link test), for compute_test_ms per format
     int sync_test_at_start = 0;                      // likewise for the synchronization self-test (after the
                                                      // half-precision test), for compute_test_ms per format
+    int l1_test_at_start = 0;                        // likewise for the L1 self-test (after the synchronization
+                                                     // test), for compute_test_ms per format
     bool version = false;
     bool labels_mode = false, reconcile = false, patch = false;
     std::string labels;                              // csv of generator names, or "all"
@@ -119,6 +121,7 @@ bool parse_flags(int argc, char** argv, Flags& f, std::string& err) {
         else if (name == "l2_test_at_start") f.l2_test_at_start = atoi(val.c_str());
         else if (name == "half_test_at_start") f.half_test_at_start = atoi(val.c_str());
         else if (name == "sync_test_at_start") f.sync_test_at_start = atoi(val.c_str());
+        else if (name == "l1_test_at_start") f.l1_test_at_start = atoi(val.c_str());
         else if (name == "hostlink_test_at_start") f.hostlink_test_at_start = atoi(val.c_str());
         else if (name == "labels") { f.labels_mode = true; f.labels = val; }
         else { err = "flag provided but not defined: -" + name; return false; }
@@ -798,6 +801,32 @@ void run_sync_test(b2dp_ctx* ctx, const Flags& fl) {
     }
 }
 
+// -l1_test_at_start=1: likewise for the L1 self-test (the L1 data cache, the texture and read-only paths and the
+// constant cache against host-built data), after the synchronization test, for -compute_test_ms per format.
+void run_l1_test(b2dp_ctx* ctx, const Flags& fl) {
+    b2dp_compute_test_opts o{};
+    o.duration_ms = fl.compute_test_ms;
+    o.fault_sm = -1;
+    if (fl.l1_test_at_start >= 2) o.flags |= B2DP_CT_EVEN_IF_BUSY;
+    b2dp_compute_test_result res[64];
+    int n = 0;
+    const int rc = b2dp_l1_test(ctx, -1, &o, res, 64, &n);
+    if (rc != B2DP_OK) {
+        logf("L1 test at start not run: %s (%s)", b2dp_strerror(rc), b2dp_last_error(ctx));
+        return;
+    }
+    std::vector<b2dp_device> devs(n > 0 ? n : 1);
+    int nd = 0;
+    if (b2dp_enumerate(ctx, devs.data(), (int)devs.size(), &nd) != B2DP_OK) nd = 0;
+    for (int i = 0; i < n; ++i) {
+        const b2dp_compute_test_result& r = res[i];
+        logf("L1 test %s: %s, flags 0x%x, SMs %d/%d, mismatches %llu/%llu/%llu, first bad SM %d, %.2f/%.2f/%.2f "
+             "TB/s", r.device < nd ? devs[r.device].id : "?", r.healthy ? "Healthy" : "Unhealthy", r.flags,
+             r.sms_covered, r.sm_count, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
+             (unsigned long long)r.mismatches[2], r.first_bad_sm, r.tflops[0], r.tflops[1], r.tflops[2]);
+    }
+}
+
 }  // namespace
 
 int main(int argc, char** argv) {
@@ -839,6 +868,7 @@ int main(int argc, char** argv) {
     if (fl.hostlink_test_at_start) run_hostlink_test(ctx, fl);
     if (fl.half_test_at_start) run_half_test(ctx, fl);
     if (fl.sync_test_at_start) run_sync_test(ctx, fl);
+    if (fl.l1_test_at_start) run_l1_test(ctx, fl);
     char names[64][64];
     int n_res = 0;
     rc = b2dp_resource_list(ctx, fl.strategy.c_str(), names, 64, &n_res);  // main.go:141-146

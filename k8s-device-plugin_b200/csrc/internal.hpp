@@ -147,7 +147,7 @@ void cuda_set_health_event_callback(CudaBackend*, std::function<void()> fn);
 // a build of the library whose backend has none (the CPU-only build of ctx.cpp the sanitizer tests link against a
 // stand-in backend) simply leaves these null, and b2dp_memtest / b2dp_compute_test / b2dp_fp_test / b2dp_sfu_test /
 // b2dp_smem_test / b2dp_regfile_test / b2dp_int_test / b2dp_l2_test / b2dp_hostlink_test / b2dp_half_test /
-// b2dp_sync_test then return B2DP_E_UNSUPPORTED.
+// b2dp_sync_test / b2dp_l1_test then return B2DP_E_UNSUPPORTED.
 // cuda_backend.cu fills them in during static initialisation.
 struct DiagHooks {
     // b2dp_memtest on `device` (-1 = all); B2DP_E_UNSUPPORTED without the in-process probe
@@ -187,6 +187,9 @@ struct DiagHooks {
     // b2dp_sync_test on `device` (-1 = all); B2DP_E_UNSUPPORTED without the in-process probe
     int (*sync_test)(CudaBackend*, int device, const b2dp_compute_test_opts* opts,
                      std::vector<b2dp_compute_test_result>& out, std::string& err) = nullptr;
+    // b2dp_l1_test on `device` (-1 = all); B2DP_E_UNSUPPORTED without the in-process probe
+    int (*l1_test)(CudaBackend*, int device, const b2dp_compute_test_opts* opts,
+                   std::vector<b2dp_compute_test_result>& out, std::string& err) = nullptr;
 };
 DiagHooks& diag_hooks();  // ctx.cpp
 

@@ -11,6 +11,7 @@
 //                            | fp_test [duration_ms] | sfu_test [duration_ms] | smem_test [duration_ms]
 //                            | regfile_test [duration_ms] | int_test [duration_ms] | l2_test [duration_ms]
 //                            | hostlink_test [duration_ms] | half_test [duration_ms] | sync_test [duration_ms]
+//                            | l1_test [duration_ms]
 #include <algorithm>
 #include <chrono>
 #include <ctime>
@@ -340,6 +341,28 @@ int main(int argc, char** argv) {
             printf("%s %s err=%d flags=0x%x sms=%d/%d nsmid=%d mismatches=%llu,%llu,%llu first_bad_sm=%d "
                    "first_bad_format=%d first_bad_tile=%d ms=%.1f,%.1f,%.1f gops_atom=%.2f "
                    "gops_bar=%.2f tresults_warp=%.2f\n",
+                   devs[r.device].id, r.healthy ? "Healthy" : "Unhealthy", r.err, r.flags, r.sms_covered, r.sm_count,
+                   r.nsmid, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
+                   (unsigned long long)r.mismatches[2], r.first_bad_sm, r.first_bad_format, r.first_bad_tile, r.ms[0],
+                   r.ms[1], r.ms[2], r.tflops[0], r.tflops[1], r.tflops[2]);
+            bad += !r.healthy;
+        }
+        b2dp_close(ctx);
+        return bad ? 1 : 0;
+    } else if (cmd == "l1_test") {  // one line per device; exit status 1 if any device is Unhealthy
+        b2dp_compute_test_opts co{};
+        co.duration_ms = argc > 3 ? (uint32_t)strtoul(argv[3], nullptr, 0) : 0;
+        co.fault_sm = -1;
+        std::vector<b2dp_compute_test_result> res(n ? n : 1);
+        int m = 0;
+        if ((rc = b2dp_l1_test(ctx, -1, &co, res.data(), (int)res.size(), &m)) != B2DP_OK)
+            return die(ctx, "b2dp_l1_test", rc);
+        int bad = 0;
+        for (int i = 0; i < m; ++i) {
+            const b2dp_compute_test_result& r = res[i];
+            printf("%s %s err=%d flags=0x%x sms=%d/%d nsmid=%d mismatches=%llu,%llu,%llu first_bad_sm=%d "
+                   "first_bad_format=%d first_bad_tile=%d ms=%.1f,%.1f,%.1f tbs_data=%.2f "
+                   "tbs_tex=%.2f tbs_const=%.2f\n",
                    devs[r.device].id, r.healthy ? "Healthy" : "Unhealthy", r.err, r.flags, r.sms_covered, r.sm_count,
                    r.nsmid, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
                    (unsigned long long)r.mismatches[2], r.first_bad_sm, r.first_bad_format, r.first_bad_tile, r.ms[0],
