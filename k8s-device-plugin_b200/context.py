@@ -242,19 +242,23 @@ class Context:
                               r.free_before, r.total_memory, list(r.mismatches), r.first_bad_word, r.ecc_corrected,
                               r.ecc_uncorrected, r.ms, r.gbs) for r in arr[:n]]
 
+    def _sm_test(self, fn, device, duration_ms, timeout_ms, even_if_busy, fault_sm, fault_mask) -> List[ComputeTestResult]:
+        """One SM self-test through its entry point `fn`: the ten share their options and result structs."""
+        opts = N.ComputeTestOpts(duration_ms, timeout_ms, N.CT_EVEN_IF_BUSY if even_if_busy else 0, fault_sm, fault_mask, 0)
+        rc, arr, n = N.grow_call(lambda cap: (N.ComputeTestResult * cap)(),
+                                 lambda a, cap, pn: fn(self._h, device, C.byref(opts), a, cap, pn))
+        N.check(rc, self._h)
+        return [ComputeTestResult(r.device, bool(r.healthy), r.err, r.flags, r.seed, r.sm_count, r.nsmid, r.sms_covered,
+                                  list(r.bad_sm_mask), list(r.mismatches), r.first_bad_sm, r.first_bad_format,
+                                  r.first_bad_tile, list(r.ms), list(r.tflops)) for r in arr[:n]]
+
     def compute_test(self, device: int = -1, duration_ms: int = 0, timeout_ms: int = 0, even_if_busy: bool = False,
                      fault_sm: int = -1, fault_mask: int = 0) -> List[ComputeTestResult]:
         """On-demand tensor-core self-test of `device` (-1 = every GPU, b2dp_compute_test): BF16, FP8 and INT8 warpgroup
         GEMMs on every SM for duration_ms each (0 = 1000), every result compared bit for bit with the host's exact
         product.  A failure is latched: later probe results carry RES_COMPUTE and are Unhealthy until probe_reset().
         fault_sm / fault_mask is a test hook that flips bits of one accumulator on the SM with that %smid."""
-        opts = N.ComputeTestOpts(duration_ms, timeout_ms, N.CT_EVEN_IF_BUSY if even_if_busy else 0, fault_sm, fault_mask, 0)
-        rc, arr, n = N.grow_call(lambda cap: (N.ComputeTestResult * cap)(),
-                                 lambda a, cap, pn: N.lib.b2dp_compute_test(self._h, device, C.byref(opts), a, cap, pn))
-        N.check(rc, self._h)
-        return [ComputeTestResult(r.device, bool(r.healthy), r.err, r.flags, r.seed, r.sm_count, r.nsmid, r.sms_covered,
-                                  list(r.bad_sm_mask), list(r.mismatches), r.first_bad_sm, r.first_bad_format,
-                                  r.first_bad_tile, list(r.ms), list(r.tflops)) for r in arr[:n]]
+        return self._sm_test(N.lib.b2dp_compute_test, device, duration_ms, timeout_ms, even_if_busy, fault_sm, fault_mask)
 
     def fp_test(self, device: int = -1, duration_ms: int = 0, timeout_ms: int = 0, even_if_busy: bool = False,
                 fault_sm: int = -1, fault_mask: int = 0) -> List[ComputeTestResult]:
@@ -262,13 +266,7 @@ class Context:
         for duration_ms each (0 = 1000), every result compared bit for bit with the host's IEEE 754 result.  The
         per-format lists are indexed by FT_FP32, FT_FP64, FT_DMMA.  A failure is latched like compute_test()'s
         (RES_COMPUTE until probe_reset()); fault_sm / fault_mask flips bits of one result on the SM with that %smid."""
-        opts = N.ComputeTestOpts(duration_ms, timeout_ms, N.CT_EVEN_IF_BUSY if even_if_busy else 0, fault_sm, fault_mask, 0)
-        rc, arr, n = N.grow_call(lambda cap: (N.ComputeTestResult * cap)(),
-                                 lambda a, cap, pn: N.lib.b2dp_fp_test(self._h, device, C.byref(opts), a, cap, pn))
-        N.check(rc, self._h)
-        return [ComputeTestResult(r.device, bool(r.healthy), r.err, r.flags, r.seed, r.sm_count, r.nsmid, r.sms_covered,
-                                  list(r.bad_sm_mask), list(r.mismatches), r.first_bad_sm, r.first_bad_format,
-                                  r.first_bad_tile, list(r.ms), list(r.tflops)) for r in arr[:n]]
+        return self._sm_test(N.lib.b2dp_fp_test, device, duration_ms, timeout_ms, even_if_busy, fault_sm, fault_mask)
 
     def sfu_test(self, device: int = -1, duration_ms: int = 0, timeout_ms: int = 0, even_if_busy: bool = False,
                  fault_sm: int = -1, fault_mask: int = 0) -> List[ComputeTestResult]:
@@ -278,13 +276,7 @@ class Context:
         lists are indexed by SF_F32, SF_ROOT, SF_F16; flags may carry CT_NO_CONSENSUS / CT_OUT_OF_BOUND.  A failure is
         latched like compute_test()'s (RES_COMPUTE until probe_reset()); fault_sm / fault_mask flips bits of one result
         on the SM with that %smid, in both launches."""
-        opts = N.ComputeTestOpts(duration_ms, timeout_ms, N.CT_EVEN_IF_BUSY if even_if_busy else 0, fault_sm, fault_mask, 0)
-        rc, arr, n = N.grow_call(lambda cap: (N.ComputeTestResult * cap)(),
-                                 lambda a, cap, pn: N.lib.b2dp_sfu_test(self._h, device, C.byref(opts), a, cap, pn))
-        N.check(rc, self._h)
-        return [ComputeTestResult(r.device, bool(r.healthy), r.err, r.flags, r.seed, r.sm_count, r.nsmid, r.sms_covered,
-                                  list(r.bad_sm_mask), list(r.mismatches), r.first_bad_sm, r.first_bad_format,
-                                  r.first_bad_tile, list(r.ms), list(r.tflops)) for r in arr[:n]]
+        return self._sm_test(N.lib.b2dp_sfu_test, device, duration_ms, timeout_ms, even_if_busy, fault_sm, fault_mask)
 
     def smem_test(self, device: int = -1, duration_ms: int = 0, timeout_ms: int = 0, even_if_busy: bool = False,
                   fault_sm: int = -1, fault_mask: int = 0) -> List[ComputeTestResult]:
@@ -293,13 +285,7 @@ class Context:
         lists are indexed by SH_WORD, SH_BYTE, SH_DSMEM; tflops holds TB/s; flags may carry CT_ECC_CORRECTED / CT_ECC /
         CT_NO_ECC.  A failure is latched like compute_test()'s (RES_COMPUTE until probe_reset()); fault_sm / fault_mask
         flips bits of one word of the array of the SM with that %smid, in the first comparison."""
-        opts = N.ComputeTestOpts(duration_ms, timeout_ms, N.CT_EVEN_IF_BUSY if even_if_busy else 0, fault_sm, fault_mask, 0)
-        rc, arr, n = N.grow_call(lambda cap: (N.ComputeTestResult * cap)(),
-                                 lambda a, cap, pn: N.lib.b2dp_smem_test(self._h, device, C.byref(opts), a, cap, pn))
-        N.check(rc, self._h)
-        return [ComputeTestResult(r.device, bool(r.healthy), r.err, r.flags, r.seed, r.sm_count, r.nsmid, r.sms_covered,
-                                  list(r.bad_sm_mask), list(r.mismatches), r.first_bad_sm, r.first_bad_format,
-                                  r.first_bad_tile, list(r.ms), list(r.tflops)) for r in arr[:n]]
+        return self._sm_test(N.lib.b2dp_smem_test, device, duration_ms, timeout_ms, even_if_busy, fault_sm, fault_mask)
 
     def regfile_test(self, device: int = -1, duration_ms: int = 0, timeout_ms: int = 0, even_if_busy: bool = False,
                      fault_sm: int = -1, fault_mask: int = 0) -> List[ComputeTestResult]:
@@ -308,13 +294,7 @@ class Context:
         are indexed by RF_ALU, RF_LOAD, RF_HOLD; tflops holds TB/s of register data; flags may carry CT_ECC_CORRECTED /
         CT_ECC / CT_NO_ECC.  A failure is latched like compute_test()'s (RES_COMPUTE until probe_reset()); fault_sm /
         fault_mask flips bits of one held register of one thread of the SM with that %smid, in the first comparison."""
-        opts = N.ComputeTestOpts(duration_ms, timeout_ms, N.CT_EVEN_IF_BUSY if even_if_busy else 0, fault_sm, fault_mask, 0)
-        rc, arr, n = N.grow_call(lambda cap: (N.ComputeTestResult * cap)(),
-                                 lambda a, cap, pn: N.lib.b2dp_regfile_test(self._h, device, C.byref(opts), a, cap, pn))
-        N.check(rc, self._h)
-        return [ComputeTestResult(r.device, bool(r.healthy), r.err, r.flags, r.seed, r.sm_count, r.nsmid, r.sms_covered,
-                                  list(r.bad_sm_mask), list(r.mismatches), r.first_bad_sm, r.first_bad_format,
-                                  r.first_bad_tile, list(r.ms), list(r.tflops)) for r in arr[:n]]
+        return self._sm_test(N.lib.b2dp_regfile_test, device, duration_ms, timeout_ms, even_if_busy, fault_sm, fault_mask)
 
     def int_test(self, device: int = -1, duration_ms: int = 0, timeout_ms: int = 0, even_if_busy: bool = False,
                  fault_sm: int = -1, fault_mask: int = 0) -> List[ComputeTestResult]:
@@ -324,13 +304,7 @@ class Context:
         per-format lists are indexed by IT_MAD, IT_BIT, IT_WARP; tflops holds T result words/s.  A failure is latched
         like compute_test()'s (RES_COMPUTE until probe_reset()); fault_sm / fault_mask flips bits of one result word of
         one thread of the SM with that %smid, in the first comparison."""
-        opts = N.ComputeTestOpts(duration_ms, timeout_ms, N.CT_EVEN_IF_BUSY if even_if_busy else 0, fault_sm, fault_mask, 0)
-        rc, arr, n = N.grow_call(lambda cap: (N.ComputeTestResult * cap)(),
-                                 lambda a, cap, pn: N.lib.b2dp_int_test(self._h, device, C.byref(opts), a, cap, pn))
-        N.check(rc, self._h)
-        return [ComputeTestResult(r.device, bool(r.healthy), r.err, r.flags, r.seed, r.sm_count, r.nsmid, r.sms_covered,
-                                  list(r.bad_sm_mask), list(r.mismatches), r.first_bad_sm, r.first_bad_format,
-                                  r.first_bad_tile, list(r.ms), list(r.tflops)) for r in arr[:n]]
+        return self._sm_test(N.lib.b2dp_int_test, device, duration_ms, timeout_ms, even_if_busy, fault_sm, fault_mask)
 
     def l2_test(self, device: int = -1, duration_ms: int = 0, timeout_ms: int = 0, even_if_busy: bool = False,
                  fault_sm: int = -1, fault_mask: int = 0) -> List[ComputeTestResult]:
@@ -340,13 +314,7 @@ class Context:
         L2_WORD, L2_BYTE, L2_ATOM; tflops holds TB/s, TB/s and G atomic ops/s.  A failure is latched like
         compute_test()'s (RES_COMPUTE until probe_reset()); fault_sm / fault_mask makes one CTA on the SM with that
         %smid flip bits of one word in the first comparison, which the CTA that reads the word next counts."""
-        opts = N.ComputeTestOpts(duration_ms, timeout_ms, N.CT_EVEN_IF_BUSY if even_if_busy else 0, fault_sm, fault_mask, 0)
-        rc, arr, n = N.grow_call(lambda cap: (N.ComputeTestResult * cap)(),
-                                 lambda a, cap, pn: N.lib.b2dp_l2_test(self._h, device, C.byref(opts), a, cap, pn))
-        N.check(rc, self._h)
-        return [ComputeTestResult(r.device, bool(r.healthy), r.err, r.flags, r.seed, r.sm_count, r.nsmid, r.sms_covered,
-                                  list(r.bad_sm_mask), list(r.mismatches), r.first_bad_sm, r.first_bad_format,
-                                  r.first_bad_tile, list(r.ms), list(r.tflops)) for r in arr[:n]]
+        return self._sm_test(N.lib.b2dp_l2_test, device, duration_ms, timeout_ms, even_if_busy, fault_sm, fault_mask)
 
     def half_test(self, device: int = -1, duration_ms: int = 0, timeout_ms: int = 0, even_if_busy: bool = False,
                   fault_sm: int = -1, fault_mask: int = 0) -> List[ComputeTestResult]:
@@ -357,13 +325,7 @@ class Context:
         holds T result words/s.  A failure is latched like compute_test()'s (RES_COMPUTE until probe_reset());
         fault_sm / fault_mask flips bits of one result word of one thread of the SM with that %smid, in the first
         comparison."""
-        opts = N.ComputeTestOpts(duration_ms, timeout_ms, N.CT_EVEN_IF_BUSY if even_if_busy else 0, fault_sm, fault_mask, 0)
-        rc, arr, n = N.grow_call(lambda cap: (N.ComputeTestResult * cap)(),
-                                 lambda a, cap, pn: N.lib.b2dp_half_test(self._h, device, C.byref(opts), a, cap, pn))
-        N.check(rc, self._h)
-        return [ComputeTestResult(r.device, bool(r.healthy), r.err, r.flags, r.seed, r.sm_count, r.nsmid, r.sms_covered,
-                                  list(r.bad_sm_mask), list(r.mismatches), r.first_bad_sm, r.first_bad_format,
-                                  r.first_bad_tile, list(r.ms), list(r.tflops)) for r in arr[:n]]
+        return self._sm_test(N.lib.b2dp_half_test, device, duration_ms, timeout_ms, even_if_busy, fault_sm, fault_mask)
 
     def sync_test(self, device: int = -1, duration_ms: int = 0, timeout_ms: int = 0, even_if_busy: bool = False,
                   fault_sm: int = -1, fault_mask: int = 0) -> List[ComputeTestResult]:
@@ -373,13 +335,7 @@ class Context:
         SY_ATOM, SY_BAR, SY_WARP; tflops holds G atomic ops/s, G barrier ops/s and T result words/s.  A failure is
         latched like compute_test()'s (RES_COMPUTE until probe_reset()); fault_sm / fault_mask flips bits of one result
         word of one thread of the SM with that %smid, in the first comparison."""
-        opts = N.ComputeTestOpts(duration_ms, timeout_ms, N.CT_EVEN_IF_BUSY if even_if_busy else 0, fault_sm, fault_mask, 0)
-        rc, arr, n = N.grow_call(lambda cap: (N.ComputeTestResult * cap)(),
-                                 lambda a, cap, pn: N.lib.b2dp_sync_test(self._h, device, C.byref(opts), a, cap, pn))
-        N.check(rc, self._h)
-        return [ComputeTestResult(r.device, bool(r.healthy), r.err, r.flags, r.seed, r.sm_count, r.nsmid, r.sms_covered,
-                                  list(r.bad_sm_mask), list(r.mismatches), r.first_bad_sm, r.first_bad_format,
-                                  r.first_bad_tile, list(r.ms), list(r.tflops)) for r in arr[:n]]
+        return self._sm_test(N.lib.b2dp_sync_test, device, duration_ms, timeout_ms, even_if_busy, fault_sm, fault_mask)
 
     def l1_test(self, device: int = -1, duration_ms: int = 0, timeout_ms: int = 0, even_if_busy: bool = False,
                 fault_sm: int = -1, fault_mask: int = 0) -> List[ComputeTestResult]:
@@ -389,13 +345,7 @@ class Context:
         L1_TEX, L1_CONST; tflops holds TB/s the loads deliver (L1_DATA: and its stores).  A failure is latched like
         compute_test()'s (RES_COMPUTE until probe_reset()); fault_sm / fault_mask flips bits of one word of the span
         (L1_DATA) or of one loaded value (L1_TEX, L1_CONST) on the SM with that %smid, in the first comparison."""
-        opts = N.ComputeTestOpts(duration_ms, timeout_ms, N.CT_EVEN_IF_BUSY if even_if_busy else 0, fault_sm, fault_mask, 0)
-        rc, arr, n = N.grow_call(lambda cap: (N.ComputeTestResult * cap)(),
-                                 lambda a, cap, pn: N.lib.b2dp_l1_test(self._h, device, C.byref(opts), a, cap, pn))
-        N.check(rc, self._h)
-        return [ComputeTestResult(r.device, bool(r.healthy), r.err, r.flags, r.seed, r.sm_count, r.nsmid, r.sms_covered,
-                                  list(r.bad_sm_mask), list(r.mismatches), r.first_bad_sm, r.first_bad_format,
-                                  r.first_bad_tile, list(r.ms), list(r.tflops)) for r in arr[:n]]
+        return self._sm_test(N.lib.b2dp_l1_test, device, duration_ms, timeout_ms, even_if_busy, fault_sm, fault_mask)
 
     def hostlink_test(self, device: int = -1, bytes: int = 0, duration_ms: int = 0, timeout_ms: int = 0,
                       even_if_busy: bool = False, fault_word: int = 0, fault_mask: int = 0) -> List[HostlinkResult]:

@@ -439,268 +439,95 @@ extern "C" int b2dp_probe_peek(b2dp_ctx* c, int device, uint64_t word_index, uin
     return rc == B2DP_OK ? rc : fail(rc, err);
 }
 
-extern "C" int b2dp_memtest(b2dp_ctx* c, int device, const b2dp_memtest_opts* opts, b2dp_memtest_result* out, int cap,
-                            int* n) {
+// The on-demand diagnostics' entry prologue, shared by b2dp_memtest, every b2dp_<x>_test and b2dp_hostlink_test.
+// The capacity is checked before the test runs: its results cannot be produced a second time for free.  `have` says
+// whether the backend registered the test's hook; run(results, err) calls it.
+template <class Result, class Run>
+static int diag_entry(b2dp_ctx* c, int device, Result* out, int cap, int* n, const char* name, bool have,
+                      const Run& run) {
     if (!c || !n || cap < 0) return B2DP_E_INVAL;
     if (c->kind != b2dp_ctx::CUDA)
-        return fail(B2DP_E_UNSUPPORTED, "the memory test needs the cuda: backend (there is no CPU fallback)");
-    // the capacity is checked before the test runs: its results cannot be produced a second time for free
+        return fail(B2DP_E_UNSUPPORTED, std::string("the ") + name + " needs the cuda: backend (there is no CPU fallback)");
     const int count = cuda_device_count(c->cuda);
     if (device < -1 || device >= count) return fail(B2DP_E_INVAL, "device index out of range");
     *n = device < 0 ? count : 1;
     if (*n > cap) return B2DP_E_NOSPC;
     if (*n && !out) return B2DP_E_INVAL;
-    std::vector<b2dp_memtest_result> res;
+    if (!have) return fail(B2DP_E_UNSUPPORTED, std::string("this build of the library has no ") + name);
+    std::vector<Result> res;
     std::string err;
-    const DiagHooks& dh = diag_hooks();
-    if (!dh.memtest) return fail(B2DP_E_UNSUPPORTED, "this build of the library has no memory test");
-    int rc = dh.memtest(c->cuda, device, opts, res, err);
+    int rc = run(res, err);
     if (rc != B2DP_OK) return fail(rc, err);
     *n = (int)res.size();
-    memcpy(out, res.data(), res.size() * sizeof(b2dp_memtest_result));
+    memcpy(out, res.data(), res.size() * sizeof(Result));
     return B2DP_OK;
+}
+
+extern "C" int b2dp_memtest(b2dp_ctx* c, int device, const b2dp_memtest_opts* opts, b2dp_memtest_result* out, int cap,
+                            int* n) {
+    const DiagHooks& dh = diag_hooks();
+    return diag_entry(c, device, out, cap, n, "memory test", dh.memtest != nullptr,
+                      [&](std::vector<b2dp_memtest_result>& res, std::string& err) {
+                          return dh.memtest(c->cuda, device, opts, res, err);
+                      });
+}
+
+static int sm_test_entry(SmTest t, b2dp_ctx* c, int device, const b2dp_compute_test_opts* opts,
+                         b2dp_compute_test_result* out, int cap, int* n) {
+    const DiagHooks& dh = diag_hooks();
+    return diag_entry(c, device, out, cap, n, kSmTestNames[t], dh.sm_test != nullptr,
+                      [&](std::vector<b2dp_compute_test_result>& res, std::string& err) {
+                          return dh.sm_test(c->cuda, t, device, opts, res, err);
+                      });
 }
 
 extern "C" int b2dp_compute_test(b2dp_ctx* c, int device, const b2dp_compute_test_opts* opts,
                                  b2dp_compute_test_result* out, int cap, int* n) {
-    if (!c || !n || cap < 0) return B2DP_E_INVAL;
-    if (c->kind != b2dp_ctx::CUDA)
-        return fail(B2DP_E_UNSUPPORTED, "the compute self-test needs the cuda: backend (there is no CPU fallback)");
-    // the capacity is checked before the test runs: its results cannot be produced a second time for free
-    const int count = cuda_device_count(c->cuda);
-    if (device < -1 || device >= count) return fail(B2DP_E_INVAL, "device index out of range");
-    *n = device < 0 ? count : 1;
-    if (*n > cap) return B2DP_E_NOSPC;
-    if (*n && !out) return B2DP_E_INVAL;
-    std::vector<b2dp_compute_test_result> res;
-    std::string err;
-    const DiagHooks& dh = diag_hooks();
-    if (!dh.compute_test) return fail(B2DP_E_UNSUPPORTED, "this build of the library has no compute self-test");
-    int rc = dh.compute_test(c->cuda, device, opts, res, err);
-    if (rc != B2DP_OK) return fail(rc, err);
-    *n = (int)res.size();
-    memcpy(out, res.data(), res.size() * sizeof(b2dp_compute_test_result));
-    return B2DP_OK;
+    return sm_test_entry(SM_COMPUTE, c, device, opts, out, cap, n);
 }
-
-extern "C" int b2dp_fp_test(b2dp_ctx* c, int device, const b2dp_compute_test_opts* opts, b2dp_compute_test_result* out,
-                            int cap, int* n) {
-    if (!c || !n || cap < 0) return B2DP_E_INVAL;
-    if (c->kind != b2dp_ctx::CUDA)
-        return fail(B2DP_E_UNSUPPORTED, "the FP self-test needs the cuda: backend (there is no CPU fallback)");
-    // the capacity is checked before the test runs: its results cannot be produced a second time for free
-    const int count = cuda_device_count(c->cuda);
-    if (device < -1 || device >= count) return fail(B2DP_E_INVAL, "device index out of range");
-    *n = device < 0 ? count : 1;
-    if (*n > cap) return B2DP_E_NOSPC;
-    if (*n && !out) return B2DP_E_INVAL;
-    std::vector<b2dp_compute_test_result> res;
-    std::string err;
-    const DiagHooks& dh = diag_hooks();
-    if (!dh.fp_test) return fail(B2DP_E_UNSUPPORTED, "this build of the library has no FP self-test");
-    int rc = dh.fp_test(c->cuda, device, opts, res, err);
-    if (rc != B2DP_OK) return fail(rc, err);
-    *n = (int)res.size();
-    memcpy(out, res.data(), res.size() * sizeof(b2dp_compute_test_result));
-    return B2DP_OK;
+extern "C" int b2dp_fp_test(b2dp_ctx* c, int device, const b2dp_compute_test_opts* opts,
+                            b2dp_compute_test_result* out, int cap, int* n) {
+    return sm_test_entry(SM_FP, c, device, opts, out, cap, n);
 }
-
-extern "C" int b2dp_sfu_test(b2dp_ctx* c, int device, const b2dp_compute_test_opts* opts, b2dp_compute_test_result* out,
-                             int cap, int* n) {
-    if (!c || !n || cap < 0) return B2DP_E_INVAL;
-    if (c->kind != b2dp_ctx::CUDA)
-        return fail(B2DP_E_UNSUPPORTED, "the SFU self-test needs the cuda: backend (there is no CPU fallback)");
-    // the capacity is checked before the test runs: its results cannot be produced a second time for free
-    const int count = cuda_device_count(c->cuda);
-    if (device < -1 || device >= count) return fail(B2DP_E_INVAL, "device index out of range");
-    *n = device < 0 ? count : 1;
-    if (*n > cap) return B2DP_E_NOSPC;
-    if (*n && !out) return B2DP_E_INVAL;
-    std::vector<b2dp_compute_test_result> res;
-    std::string err;
-    const DiagHooks& dh = diag_hooks();
-    if (!dh.sfu_test) return fail(B2DP_E_UNSUPPORTED, "this build of the library has no SFU self-test");
-    int rc = dh.sfu_test(c->cuda, device, opts, res, err);
-    if (rc != B2DP_OK) return fail(rc, err);
-    *n = (int)res.size();
-    memcpy(out, res.data(), res.size() * sizeof(b2dp_compute_test_result));
-    return B2DP_OK;
+extern "C" int b2dp_sfu_test(b2dp_ctx* c, int device, const b2dp_compute_test_opts* opts,
+                             b2dp_compute_test_result* out, int cap, int* n) {
+    return sm_test_entry(SM_SFU, c, device, opts, out, cap, n);
 }
-
-extern "C" int b2dp_smem_test(b2dp_ctx* c, int device, const b2dp_compute_test_opts* opts, b2dp_compute_test_result* out,
-                              int cap, int* n) {
-    if (!c || !n || cap < 0) return B2DP_E_INVAL;
-    if (c->kind != b2dp_ctx::CUDA)
-        return fail(B2DP_E_UNSUPPORTED, "the shared-memory self-test needs the cuda: backend (there is no CPU fallback)");
-    // the capacity is checked before the test runs: its results cannot be produced a second time for free
-    const int count = cuda_device_count(c->cuda);
-    if (device < -1 || device >= count) return fail(B2DP_E_INVAL, "device index out of range");
-    *n = device < 0 ? count : 1;
-    if (*n > cap) return B2DP_E_NOSPC;
-    if (*n && !out) return B2DP_E_INVAL;
-    std::vector<b2dp_compute_test_result> res;
-    std::string err;
-    const DiagHooks& dh = diag_hooks();
-    if (!dh.smem_test) return fail(B2DP_E_UNSUPPORTED, "this build of the library has no shared-memory self-test");
-    int rc = dh.smem_test(c->cuda, device, opts, res, err);
-    if (rc != B2DP_OK) return fail(rc, err);
-    *n = (int)res.size();
-    memcpy(out, res.data(), res.size() * sizeof(b2dp_compute_test_result));
-    return B2DP_OK;
+extern "C" int b2dp_smem_test(b2dp_ctx* c, int device, const b2dp_compute_test_opts* opts,
+                              b2dp_compute_test_result* out, int cap, int* n) {
+    return sm_test_entry(SM_SMEM, c, device, opts, out, cap, n);
 }
-
 extern "C" int b2dp_regfile_test(b2dp_ctx* c, int device, const b2dp_compute_test_opts* opts,
                                  b2dp_compute_test_result* out, int cap, int* n) {
-    if (!c || !n || cap < 0) return B2DP_E_INVAL;
-    if (c->kind != b2dp_ctx::CUDA)
-        return fail(B2DP_E_UNSUPPORTED, "the register-file self-test needs the cuda: backend (there is no CPU fallback)");
-    // the capacity is checked before the test runs: its results cannot be produced a second time for free
-    const int count = cuda_device_count(c->cuda);
-    if (device < -1 || device >= count) return fail(B2DP_E_INVAL, "device index out of range");
-    *n = device < 0 ? count : 1;
-    if (*n > cap) return B2DP_E_NOSPC;
-    if (*n && !out) return B2DP_E_INVAL;
-    std::vector<b2dp_compute_test_result> res;
-    std::string err;
-    const DiagHooks& dh = diag_hooks();
-    if (!dh.regfile_test) return fail(B2DP_E_UNSUPPORTED, "this build of the library has no register-file self-test");
-    int rc = dh.regfile_test(c->cuda, device, opts, res, err);
-    if (rc != B2DP_OK) return fail(rc, err);
-    *n = (int)res.size();
-    memcpy(out, res.data(), res.size() * sizeof(b2dp_compute_test_result));
-    return B2DP_OK;
+    return sm_test_entry(SM_REGFILE, c, device, opts, out, cap, n);
 }
-
 extern "C" int b2dp_int_test(b2dp_ctx* c, int device, const b2dp_compute_test_opts* opts,
                              b2dp_compute_test_result* out, int cap, int* n) {
-    if (!c || !n || cap < 0) return B2DP_E_INVAL;
-    if (c->kind != b2dp_ctx::CUDA)
-        return fail(B2DP_E_UNSUPPORTED, "the integer self-test needs the cuda: backend (there is no CPU fallback)");
-    // the capacity is checked before the test runs: its results cannot be produced a second time for free
-    const int count = cuda_device_count(c->cuda);
-    if (device < -1 || device >= count) return fail(B2DP_E_INVAL, "device index out of range");
-    *n = device < 0 ? count : 1;
-    if (*n > cap) return B2DP_E_NOSPC;
-    if (*n && !out) return B2DP_E_INVAL;
-    std::vector<b2dp_compute_test_result> res;
-    std::string err;
-    const DiagHooks& dh = diag_hooks();
-    if (!dh.int_test) return fail(B2DP_E_UNSUPPORTED, "this build of the library has no integer self-test");
-    int rc = dh.int_test(c->cuda, device, opts, res, err);
-    if (rc != B2DP_OK) return fail(rc, err);
-    *n = (int)res.size();
-    memcpy(out, res.data(), res.size() * sizeof(b2dp_compute_test_result));
-    return B2DP_OK;
+    return sm_test_entry(SM_INT, c, device, opts, out, cap, n);
 }
-
 extern "C" int b2dp_l2_test(b2dp_ctx* c, int device, const b2dp_compute_test_opts* opts,
                             b2dp_compute_test_result* out, int cap, int* n) {
-    if (!c || !n || cap < 0) return B2DP_E_INVAL;
-    if (c->kind != b2dp_ctx::CUDA)
-        return fail(B2DP_E_UNSUPPORTED, "the L2 self-test needs the cuda: backend (there is no CPU fallback)");
-    // the capacity is checked before the test runs: its results cannot be produced a second time for free
-    const int count = cuda_device_count(c->cuda);
-    if (device < -1 || device >= count) return fail(B2DP_E_INVAL, "device index out of range");
-    *n = device < 0 ? count : 1;
-    if (*n > cap) return B2DP_E_NOSPC;
-    if (*n && !out) return B2DP_E_INVAL;
-    std::vector<b2dp_compute_test_result> res;
-    std::string err;
-    const DiagHooks& dh = diag_hooks();
-    if (!dh.l2_test) return fail(B2DP_E_UNSUPPORTED, "this build of the library has no L2 self-test");
-    int rc = dh.l2_test(c->cuda, device, opts, res, err);
-    if (rc != B2DP_OK) return fail(rc, err);
-    *n = (int)res.size();
-    memcpy(out, res.data(), res.size() * sizeof(b2dp_compute_test_result));
-    return B2DP_OK;
+    return sm_test_entry(SM_L2, c, device, opts, out, cap, n);
 }
-
 extern "C" int b2dp_hostlink_test(b2dp_ctx* c, int device, const b2dp_hostlink_opts* opts, b2dp_hostlink_result* out,
                                   int cap, int* n) {
-    if (!c || !n || cap < 0) return B2DP_E_INVAL;
-    if (c->kind != b2dp_ctx::CUDA)
-        return fail(B2DP_E_UNSUPPORTED, "the host-link self-test needs the cuda: backend (there is no CPU fallback)");
-    // the capacity is checked before the test runs: its results cannot be produced a second time for free
-    const int count = cuda_device_count(c->cuda);
-    if (device < -1 || device >= count) return fail(B2DP_E_INVAL, "device index out of range");
-    *n = device < 0 ? count : 1;
-    if (*n > cap) return B2DP_E_NOSPC;
-    if (*n && !out) return B2DP_E_INVAL;
-    std::vector<b2dp_hostlink_result> res;
-    std::string err;
     const DiagHooks& dh = diag_hooks();
-    if (!dh.hostlink_test) return fail(B2DP_E_UNSUPPORTED, "this build of the library has no host-link self-test");
-    int rc = dh.hostlink_test(c->cuda, device, opts, res, err);
-    if (rc != B2DP_OK) return fail(rc, err);
-    *n = (int)res.size();
-    memcpy(out, res.data(), res.size() * sizeof(b2dp_hostlink_result));
-    return B2DP_OK;
+    return diag_entry(c, device, out, cap, n, "host-link self-test", dh.hostlink_test != nullptr,
+                      [&](std::vector<b2dp_hostlink_result>& res, std::string& err) {
+                          return dh.hostlink_test(c->cuda, device, opts, res, err);
+                      });
 }
-
 extern "C" int b2dp_half_test(b2dp_ctx* c, int device, const b2dp_compute_test_opts* opts,
                               b2dp_compute_test_result* out, int cap, int* n) {
-    if (!c || !n || cap < 0) return B2DP_E_INVAL;
-    if (c->kind != b2dp_ctx::CUDA)
-        return fail(B2DP_E_UNSUPPORTED, "the half-precision self-test needs the cuda: backend (there is no CPU fallback)");
-    // the capacity is checked before the test runs: its results cannot be produced a second time for free
-    const int count = cuda_device_count(c->cuda);
-    if (device < -1 || device >= count) return fail(B2DP_E_INVAL, "device index out of range");
-    *n = device < 0 ? count : 1;
-    if (*n > cap) return B2DP_E_NOSPC;
-    if (*n && !out) return B2DP_E_INVAL;
-    std::vector<b2dp_compute_test_result> res;
-    std::string err;
-    const DiagHooks& dh = diag_hooks();
-    if (!dh.half_test) return fail(B2DP_E_UNSUPPORTED, "this build of the library has no half-precision self-test");
-    int rc = dh.half_test(c->cuda, device, opts, res, err);
-    if (rc != B2DP_OK) return fail(rc, err);
-    *n = (int)res.size();
-    memcpy(out, res.data(), res.size() * sizeof(b2dp_compute_test_result));
-    return B2DP_OK;
+    return sm_test_entry(SM_HALF, c, device, opts, out, cap, n);
 }
-
 extern "C" int b2dp_sync_test(b2dp_ctx* c, int device, const b2dp_compute_test_opts* opts,
                               b2dp_compute_test_result* out, int cap, int* n) {
-    if (!c || !n || cap < 0) return B2DP_E_INVAL;
-    if (c->kind != b2dp_ctx::CUDA)
-        return fail(B2DP_E_UNSUPPORTED, "the synchronization self-test needs the cuda: backend (there is no CPU fallback)");
-    // the capacity is checked before the test runs: its results cannot be produced a second time for free
-    const int count = cuda_device_count(c->cuda);
-    if (device < -1 || device >= count) return fail(B2DP_E_INVAL, "device index out of range");
-    *n = device < 0 ? count : 1;
-    if (*n > cap) return B2DP_E_NOSPC;
-    if (*n && !out) return B2DP_E_INVAL;
-    std::vector<b2dp_compute_test_result> res;
-    std::string err;
-    const DiagHooks& dh = diag_hooks();
-    if (!dh.sync_test) return fail(B2DP_E_UNSUPPORTED, "this build of the library has no synchronization self-test");
-    int rc = dh.sync_test(c->cuda, device, opts, res, err);
-    if (rc != B2DP_OK) return fail(rc, err);
-    *n = (int)res.size();
-    memcpy(out, res.data(), res.size() * sizeof(b2dp_compute_test_result));
-    return B2DP_OK;
+    return sm_test_entry(SM_SYNC, c, device, opts, out, cap, n);
 }
-
 extern "C" int b2dp_l1_test(b2dp_ctx* c, int device, const b2dp_compute_test_opts* opts,
                             b2dp_compute_test_result* out, int cap, int* n) {
-    if (!c || !n || cap < 0) return B2DP_E_INVAL;
-    if (c->kind != b2dp_ctx::CUDA)
-        return fail(B2DP_E_UNSUPPORTED, "the L1 self-test needs the cuda: backend (there is no CPU fallback)");
-    // the capacity is checked before the test runs: its results cannot be produced a second time for free
-    const int count = cuda_device_count(c->cuda);
-    if (device < -1 || device >= count) return fail(B2DP_E_INVAL, "device index out of range");
-    *n = device < 0 ? count : 1;
-    if (*n > cap) return B2DP_E_NOSPC;
-    if (*n && !out) return B2DP_E_INVAL;
-    std::vector<b2dp_compute_test_result> res;
-    std::string err;
-    const DiagHooks& dh = diag_hooks();
-    if (!dh.l1_test) return fail(B2DP_E_UNSUPPORTED, "this build of the library has no L1 self-test");
-    int rc = dh.l1_test(c->cuda, device, opts, res, err);
-    if (rc != B2DP_OK) return fail(rc, err);
-    *n = (int)res.size();
-    memcpy(out, res.data(), res.size() * sizeof(b2dp_compute_test_result));
-    return B2DP_OK;
+    return sm_test_entry(SM_L1, c, device, opts, out, cap, n);
 }
 
 extern "C" int b2dp_merge_health(const char (*ids)[64], int n, int32_t default_healthy, int have_source,

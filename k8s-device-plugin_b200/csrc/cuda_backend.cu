@@ -1594,20 +1594,15 @@ static int cuda_memtest(CudaBackend* be, int device, const b2dp_memtest_opts* op
     return B2DP_OK;
 }
 
-// ---- on-demand compute self-tests (b2dp_compute_test, b2dp_fp_test, b2dp_sfu_test, b2dp_smem_test,
-// b2dp_regfile_test, b2dp_int_test, b2dp_l2_test, b2dp_half_test, b2dp_sync_test, b2dp_l1_test) ------------------
-// One launch per format on one GPU, on that GPU's worker: tc_selftest.cuh (tensor cores: BF16, FP8, INT8),
-// fp_selftest.cuh (FP32 FMA, FP64 FMA, FP64 tensor cores), sfu_selftest.cuh (the special-function unit),
-// smem_selftest.cuh (shared memory and the SM-to-SM DSMEM path), rf_selftest.cuh (the register file), int_selftest.cuh
-// (the integer pipes and the warp-exchange network), l2_selftest.cuh (the L2 and its atomic units) or half_selftest.cuh
-// (the 16-bit pipes and the type converters).  The host builds
-// every operand table and every comparison value itself (compute_test_math.hpp, fp_test_math.hpp, smem_test_math.hpp,
-// rf_test_math.hpp, int_test_math.hpp, half_test_math.hpp): a health test must not ask the device under test for its own reference values.  The SFU test departs from that rule, because no
-// bit-level model of MUFU is published: its reference step (sfu_reference) runs one CTA on every SM, takes each result
-// word's majority over the SMs, names every SM that disagrees, and bounds the majority against the exact function on
-// the host; no SM is ever judged against its own output.  The tests share this driver -- grid sizing, records, tally,
-// deadline, busy skip and the release of every allocation before the job ends, whatever happened -- through a
-// DiagSuite.
+// ---- on-demand SM self-tests (b2dp_compute_test ... b2dp_l1_test) ----------------------------------------------------
+// One launch per format on one GPU, on that GPU's worker.  Each test is a DiagSuite -- its kernels (*_selftest.cuh),
+// its host tables and checks (*_test_math.hpp) and its optional steps -- and kSuites lists them by SmTest
+// (internal.hpp).  The host builds every operand table and every comparison value itself: a health test must not ask
+// the device under test for its own reference values.  The SFU test departs from that rule, because no bit-level model
+// of MUFU is published: its reference step (sfu_reference) runs one CTA on every SM, takes each result word's majority
+// over the SMs, names every SM that disagrees, and bounds the majority against the exact function on the host; no SM
+// is ever judged against its own output.  The tests share this driver -- grid sizing, records, tally, deadline, busy
+// skip and the release of every allocation before the job ends, whatever happened.
 constexpr uint32_t kComputeTestDefaultMs = 1000;
 constexpr int kDiagScratchHeaderWords = 64;  // DiagSuite::scratch's header
 static_assert(kL2HdrWords == kDiagScratchHeaderWords, "l2_selftest's scratch header is the driver's");
@@ -1651,7 +1646,6 @@ struct DiagSuite {
     // on every SM), after the kernel's shared-memory attributes are set.  On an error it names the cause in *where.
     cudaError_t (*size_grid)(Gpu* g, int fmt, int* grid, const char** where);
     bool ecc;                                  // read NVML's volatile ECC totals around the timed launches
-    const char* test_name;                     // in the error of a backend without the test; null: by the fields above
     // Optional per-format device scratch buffer (the L2 test's spans and hot block; null: none): its size in bytes
     // for `grid` CTAs, the kDiagScratchHeaderWords header words copied to its start (the rest is zeroed), and the
     // per-CTA multiply-adds of one comparison, which depend on the buffer's size and take macs_per_tile's place.  Its
@@ -1835,7 +1829,7 @@ static cudaError_t sh_size_grid(Gpu* g, int fmt, int* grid, const char** where) 
 
 static const DiagSuite kSmemSuite = {"shared-memory test", "smem_selftest", "word/byte/dsmem", kShKernels, kShSmem,
                                      kShTableBytes, sh_suite_tile, sh_suite_half_bytes, false, nullptr,
-                                     "%.2f/%.2f/%.2f TB/s", sh_size_grid, true, "shared-memory self-test"};
+                                     "%.2f/%.2f/%.2f TB/s", sh_size_grid, true};
 
 // ---- the register-file test's suite ----
 // __launch_bounds__(kCtThreads, 2) and kRfSmemBytes each: the default grid sizing gives two CTAs on every SM, which
@@ -1852,7 +1846,7 @@ static double rf_suite_half_bytes(int fmt) { return 0.5 * rf_bytes_per_tile(fmt)
 
 static const DiagSuite kRfSuite = {"register-file test", "rf_selftest", "alu/load/hold", kRfKernels, kRfSmem,
                                    kRfTableBytes, rf_suite_tile, rf_suite_half_bytes, false, nullptr,
-                                   "%.2f/%.2f/%.2f TB/s", nullptr, true, "register-file self-test"};
+                                   "%.2f/%.2f/%.2f TB/s", nullptr, true};
 
 // ---- the integer and warp-exchange test's suite ----
 static const CtKernel kItKernels[kItFormats] = {int_selftest<IT_MAD, false>, int_selftest<IT_BIT, false>,
@@ -1868,7 +1862,7 @@ static double it_suite_half_results(int fmt) { return 0.5 * it_ops_per_tile(fmt)
 
 static const DiagSuite kIntSuite = {"integer test", "int_selftest", "mad/bit/warp", kItKernels, kItSmem, kItTableBytes,
                                     it_suite_tile, it_suite_half_results, false, nullptr,
-                                    "%.2f/%.2f/%.2f T results/s", nullptr, false, "integer self-test"};
+                                    "%.2f/%.2f/%.2f T results/s", nullptr, false};
 
 // ---- the L2 test's suite ----
 static const CtKernel kL2Kernels[kL2Formats] = {l2_selftest<L2_WORD, false>, l2_selftest<L2_BYTE, false>,
@@ -2007,7 +2001,7 @@ static void l1_unbind_suite(void* state) {
 
 static const DiagSuite kL1Suite = {"L1 test", "l1_selftest", "data/tex/const", kL1Kernels, kL1Smem, kL1TableBytesAll,
                                    l1_suite_tile, nullptr, false, nullptr, "%.2f/%.2f/%.2f TB/s", l1_size_grid, true,
-                                   "L1 self-test", l1_scratch, false, kL1Carveout, l1_bind_suite, l1_unbind_suite};
+                                   l1_scratch, false, kL1Carveout, l1_bind_suite, l1_unbind_suite};
 
 // ---- the half-precision and conversion test's suite ----
 static const CtKernel kHpKernels[kHpFormats] = {half_selftest<HP_F16, false>, half_selftest<HP_BF16, false>,
@@ -2023,7 +2017,7 @@ static double hp_suite_half_results(int fmt) { return 0.5 * hp_ops_per_tile(fmt)
 
 static const DiagSuite kHalfSuite = {"half-precision test", "half_selftest", "f16/bf16/cvt", kHpKernels, kHpSmem,
                                      kHpTableBytes, hp_suite_tile, hp_suite_half_results, false, nullptr,
-                                     "%.2f/%.2f/%.2f T results/s", nullptr, false, "half-precision self-test"};
+                                     "%.2f/%.2f/%.2f T results/s", nullptr, false};
 
 // ---- the synchronization test's suite ----
 static const CtKernel kSyKernels[kSyFormats] = {sync_selftest<SY_ATOM, false>, sync_selftest<SY_BAR, false>,
@@ -2037,12 +2031,11 @@ static void sy_suite_tile(uint32_t seed, int fmt, int tile, uint8_t* table, uint
 
 static const DiagSuite kSyncSuite = {"sync test", "sync_selftest", "atom/bar/warp", kSyKernels, kSySmem,
                                      kSyTableBytes, sy_suite_tile, sy_rate_half_units, false, nullptr,
-                                     "%.2f/%.2f/%.2f G atomic ops/s, G barrier ops/s, T results/s", nullptr, false,
-                                     "synchronization self-test"};
+                                     "%.2f/%.2f/%.2f G atomic ops/s, G barrier ops/s, T results/s", nullptr, false};
 
 static const DiagSuite kL2Suite = {"L2 test", "l2_selftest", "word/byte/atom", kL2Kernels, kL2Smem, kL2TableBytes,
                                    l2_suite_tile, nullptr, false, nullptr, "%.2f/%.2f/%.2f TB/s, TB/s, G ops/s",
-                                   l2_size_grid, true, "L2 self-test", l2_scratch, true};
+                                   l2_size_grid, true, l2_scratch, true};
 
 static std::shared_ptr<DiagTables> diag_build_tables(const DiagSuite& su, uint32_t seed) {
     auto t = std::make_shared<DiagTables>();
@@ -2237,15 +2230,11 @@ done:
     }
 }
 
-static int cuda_diag_test(const DiagSuite& su, CudaBackend* be, int device, const b2dp_compute_test_opts* opts,
-                          std::vector<b2dp_compute_test_result>& out, std::string& err) {
+static int cuda_diag_test(const DiagSuite& su, const char* name, CudaBackend* be, int device,
+                          const b2dp_compute_test_opts* opts, std::vector<b2dp_compute_test_result>& out,
+                          std::string& err) {
     if (be->units) {
-        err = std::string("the ") +
-              (su.test_name         ? su.test_name
-               : su.per_device_seed ? "compute self-test"
-               : su.reference       ? "SFU self-test"
-                                    : "FP self-test") +
-              " runs in-process only (not with probe=helpers / probe=off / MIG)";
+        err = std::string("the ") + name + " runs in-process only (not with probe=helpers / probe=off / MIG)";
         return B2DP_E_UNSUPPORTED;
     }
     if (device < -1 || device >= (int)be->gpus.size()) { err = "device index out of range"; return B2DP_E_INVAL; }
@@ -2305,54 +2294,15 @@ static int cuda_diag_test(const DiagSuite& su, CudaBackend* be, int device, cons
     return B2DP_OK;
 }
 
-static int cuda_compute_test(CudaBackend* be, int device, const b2dp_compute_test_opts* opts,
-                             std::vector<b2dp_compute_test_result>& out, std::string& err) {
-    return cuda_diag_test(kTensorSuite, be, device, opts, out, err);
-}
+// indexed by SmTest (internal.hpp)
+static const DiagSuite* const kSuites[] = {&kTensorSuite, &kFpSuite, &kSfuSuite,  &kSmemSuite, &kRfSuite,
+                                           &kIntSuite,    &kL2Suite, &kHalfSuite, &kSyncSuite, &kL1Suite};
+static_assert(sizeof kSuites / sizeof kSuites[0] == (size_t)kSmTests, "one suite per SmTest");
 
-static int cuda_fp_test(CudaBackend* be, int device, const b2dp_compute_test_opts* opts,
+static int cuda_sm_test(CudaBackend* be, int suite, int device, const b2dp_compute_test_opts* opts,
                         std::vector<b2dp_compute_test_result>& out, std::string& err) {
-    return cuda_diag_test(kFpSuite, be, device, opts, out, err);
-}
-
-static int cuda_sfu_test(CudaBackend* be, int device, const b2dp_compute_test_opts* opts,
-                         std::vector<b2dp_compute_test_result>& out, std::string& err) {
-    return cuda_diag_test(kSfuSuite, be, device, opts, out, err);
-}
-
-static int cuda_smem_test(CudaBackend* be, int device, const b2dp_compute_test_opts* opts,
-                          std::vector<b2dp_compute_test_result>& out, std::string& err) {
-    return cuda_diag_test(kSmemSuite, be, device, opts, out, err);
-}
-
-static int cuda_regfile_test(CudaBackend* be, int device, const b2dp_compute_test_opts* opts,
-                             std::vector<b2dp_compute_test_result>& out, std::string& err) {
-    return cuda_diag_test(kRfSuite, be, device, opts, out, err);
-}
-
-static int cuda_int_test(CudaBackend* be, int device, const b2dp_compute_test_opts* opts,
-                         std::vector<b2dp_compute_test_result>& out, std::string& err) {
-    return cuda_diag_test(kIntSuite, be, device, opts, out, err);
-}
-
-static int cuda_l2_test(CudaBackend* be, int device, const b2dp_compute_test_opts* opts,
-                        std::vector<b2dp_compute_test_result>& out, std::string& err) {
-    return cuda_diag_test(kL2Suite, be, device, opts, out, err);
-}
-
-static int cuda_half_test(CudaBackend* be, int device, const b2dp_compute_test_opts* opts,
-                          std::vector<b2dp_compute_test_result>& out, std::string& err) {
-    return cuda_diag_test(kHalfSuite, be, device, opts, out, err);
-}
-
-static int cuda_sync_test(CudaBackend* be, int device, const b2dp_compute_test_opts* opts,
-                          std::vector<b2dp_compute_test_result>& out, std::string& err) {
-    return cuda_diag_test(kSyncSuite, be, device, opts, out, err);
-}
-
-static int cuda_l1_test(CudaBackend* be, int device, const b2dp_compute_test_opts* opts,
-                        std::vector<b2dp_compute_test_result>& out, std::string& err) {
-    return cuda_diag_test(kL1Suite, be, device, opts, out, err);
+    if (suite < 0 || suite >= kSmTests) { err = "unknown SM self-test"; return B2DP_E_INVAL; }
+    return cuda_diag_test(*kSuites[suite], kSmTestNames[suite], be, device, opts, out, err);
 }
 
 // ---- on-demand host-link self-test (b2dp_hostlink_test) ---------------------------------------------------------------
@@ -2645,9 +2595,7 @@ static bool cuda_diag_latched(CudaBackend* be) {
 
 // registered when the library is loaded, before any entry point can run (internal.hpp DiagHooks)
 [[maybe_unused]] static const bool kDiagRegistered = [] {
-    diag_hooks() = DiagHooks{cuda_memtest, cuda_compute_test, cuda_fp_test, cuda_diag_latched, cuda_sfu_test,
-                             cuda_smem_test, cuda_regfile_test, cuda_int_test, cuda_l2_test, cuda_hostlink_test,
-                             cuda_half_test, cuda_sync_test, cuda_l1_test};
+    diag_hooks() = DiagHooks{cuda_memtest, cuda_sm_test, cuda_diag_latched, cuda_hostlink_test};
     return true;
 }();
 

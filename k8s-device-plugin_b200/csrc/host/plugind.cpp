@@ -40,6 +40,39 @@ namespace {
 
 std::atomic<bool> g_stop{false};
 
+// The SM self-tests' -<flag>=1 (2: also on GPUs another process is using): each runs on every GPU once, after open and
+// before the first registration, for -compute_test_ms per format, in this order after the memtest; the host-link test
+// runs between the L2 and half-precision tests (kSmTestsBeforeHostlink).  A failed device stays latched Unhealthy,
+// reported like a failed memtest.
+struct SmTest {
+    const char* flag;
+    const char* log;   // the log lines' prefix
+    const char* rate;  // their tflops[] columns
+    int (*run)(b2dp_ctx*, int, const b2dp_compute_test_opts*, b2dp_compute_test_result*, int, int*);
+};
+const SmTest kSmTests[] = {
+    {"compute_test_at_start", "compute test", "%.0f/%.0f/%.0f TFLOP/s", b2dp_compute_test},  // tensor cores
+    {"fp_test_at_start", "fp test", "%.1f/%.1f/%.1f TFLOP/s", b2dp_fp_test},                  // FFMA, DFMA, DMMA
+    // MUFU transcendentals, checked against the SMs' majority and host error bounds
+    {"sfu_test_at_start", "sfu test", "%.2f/%.2f/%.2f T results/s", b2dp_sfu_test},
+    // every SM's 227 KiB array and the SM-to-SM DSMEM path, marched against host patterns
+    {"smem_test_at_start", "smem test", "%.2f/%.2f/%.2f TB/s", b2dp_smem_test},
+    // 204 values per thread held in every SM's registers and marched against host patterns
+    {"regfile_test_at_start", "regfile test", "%.2f/%.2f/%.2f TB/s", b2dp_regfile_test},
+    // every SM's integer pipes and shuffle network against exact host results
+    {"int_test_at_start", "int test", "%.2f/%.2f/%.2f T results/s", b2dp_int_test},
+    // a march over an L2-resident span that moves between SMs, and the L2 atomic units, against host values
+    {"l2_test_at_start", "L2 test", "%.2f/%.2f/%.2f TB/s, TB/s, G ops/s", b2dp_l2_test},
+    // every SM's f16x2 / bf16x2 pipes and type converters against exact host results
+    {"half_test_at_start", "half test", "%.2f/%.2f/%.2f T results/s", b2dp_half_test},
+    // shared-memory atomics, barriers, mbarriers and warp collectives against the PTX ISA
+    {"sync_test_at_start", "sync test", "%.2f/%.2f/%.2f G ops/s, G ops/s, T results/s", b2dp_sync_test},
+    // the L1 data cache, the texture and read-only paths and the constant cache against host-built data
+    {"l1_test_at_start", "L1 test", "%.2f/%.2f/%.2f TB/s", b2dp_l1_test},
+};
+constexpr size_t kNumSmTests = sizeof kSmTests / sizeof kSmTests[0];
+constexpr size_t kSmTestsBeforeHostlink = 7;  // compute ... L2
+
 struct Flags {
     int pulse = 0;                                   // main.go:109
     std::string strategy = "single";                 // main.go:110
@@ -52,28 +85,9 @@ struct Flags {
     int memtest_at_start = 0;                        // 1: test the free HBM of every idle GPU before the first registration;
                                                      // 2: also GPUs another process is using
     unsigned long long memtest_max_bytes = 0;        // cap per GPU for that test (0 = all free memory above the reserve)
-    int compute_test_at_start = 0;                   // likewise for the tensor-core self-test (after the memtest if both)
-    unsigned compute_test_ms = 0;                    // its duration per format (0 = 1000 ms)
-    int fp_test_at_start = 0;                        // likewise for the FP32 / FP64 self-test (after the compute test);
-                                                     // its duration per format is compute_test_ms too
-    int sfu_test_at_start = 0;                       // likewise for the SFU self-test (after the FP test), for
-                                                     // compute_test_ms per format
-    int smem_test_at_start = 0;                      // likewise for the shared-memory self-test (after the SFU test),
-                                                     // for compute_test_ms per format
-    int regfile_test_at_start = 0;                   // likewise for the register-file self-test (after the
-                                                     // shared-memory test), for compute_test_ms per format
-    int int_test_at_start = 0;                       // likewise for the integer and warp-exchange self-test (after the
-                                                     // register-file test), for compute_test_ms per format
-    int l2_test_at_start = 0;                        // likewise for the L2 self-test (after the integer test), for
-                                                     // compute_test_ms per format
-    int hostlink_test_at_start = 0;                  // likewise for the host-link self-test (after the L2 test), for
-                                                     // compute_test_ms per format
-    int half_test_at_start = 0;                      // likewise for the half-precision and conversion self-test (after
-                                                     // the host-link test), for compute_test_ms per format
-    int sync_test_at_start = 0;                      // likewise for the synchronization self-test (after the
-                                                     // half-precision test), for compute_test_ms per format
-    int l1_test_at_start = 0;                        // likewise for the L1 self-test (after the synchronization
-                                                     // test), for compute_test_ms per format
+    unsigned compute_test_ms = 0;                    // the SM and host-link self-tests' duration per format (0 = 1000 ms)
+    int sm_test_at_start[kNumSmTests] = {};          // per kSmTests row: its -<flag> level
+    int hostlink_test_at_start = 0;                  // likewise for the host-link self-test (after the L2 test)
     bool version = false;
     bool labels_mode = false, reconcile = false, patch = false;
     std::string labels;                              // csv of generator names, or "all"
@@ -111,20 +125,15 @@ bool parse_flags(int argc, char** argv, Flags& f, std::string& err) {
         else if (name == "exporter_socket") f.exporter_socket = val;
         else if (name == "memtest_at_start") f.memtest_at_start = atoi(val.c_str());
         else if (name == "memtest_max_bytes") f.memtest_max_bytes = strtoull(val.c_str(), nullptr, 0);
-        else if (name == "compute_test_at_start") f.compute_test_at_start = atoi(val.c_str());
         else if (name == "compute_test_ms") f.compute_test_ms = (unsigned)strtoul(val.c_str(), nullptr, 0);
-        else if (name == "fp_test_at_start") f.fp_test_at_start = atoi(val.c_str());
-        else if (name == "sfu_test_at_start") f.sfu_test_at_start = atoi(val.c_str());
-        else if (name == "smem_test_at_start") f.smem_test_at_start = atoi(val.c_str());
-        else if (name == "regfile_test_at_start") f.regfile_test_at_start = atoi(val.c_str());
-        else if (name == "int_test_at_start") f.int_test_at_start = atoi(val.c_str());
-        else if (name == "l2_test_at_start") f.l2_test_at_start = atoi(val.c_str());
-        else if (name == "half_test_at_start") f.half_test_at_start = atoi(val.c_str());
-        else if (name == "sync_test_at_start") f.sync_test_at_start = atoi(val.c_str());
-        else if (name == "l1_test_at_start") f.l1_test_at_start = atoi(val.c_str());
         else if (name == "hostlink_test_at_start") f.hostlink_test_at_start = atoi(val.c_str());
         else if (name == "labels") { f.labels_mode = true; f.labels = val; }
-        else { err = "flag provided but not defined: -" + name; return false; }
+        else {
+            size_t t = 0;
+            while (t < kNumSmTests && name != kSmTests[t].flag) ++t;
+            if (t == kNumSmTests) { err = "flag provided but not defined: -" + name; return false; }
+            f.sm_test_at_start[t] = atoi(val.c_str());
+        }
     }
     if (!f.plugin_dir.empty() && f.plugin_dir.back() != '/') f.plugin_dir += '/';
     return true;
@@ -541,18 +550,18 @@ void run_memtest(b2dp_ctx* ctx, const Flags& fl) {
     }
 }
 
-// -compute_test_at_start=1: run the tensor-core self-test on every GPU once, after open (and after the memtest) and
-// before the first registration.  A failed device stays latched Unhealthy, reported like a failed memtest.
-void run_compute_test(b2dp_ctx* ctx, const Flags& fl) {
+// -<flag>=1 of kSmTests[t] (see there)
+void run_sm_test(b2dp_ctx* ctx, const Flags& fl, size_t t) {
+    const SmTest& st = kSmTests[t];
     b2dp_compute_test_opts o{};
     o.duration_ms = fl.compute_test_ms;
     o.fault_sm = -1;
-    if (fl.compute_test_at_start >= 2) o.flags |= B2DP_CT_EVEN_IF_BUSY;
+    if (fl.sm_test_at_start[t] >= 2) o.flags |= B2DP_CT_EVEN_IF_BUSY;
     b2dp_compute_test_result res[64];
     int n = 0;
-    const int rc = b2dp_compute_test(ctx, -1, &o, res, 64, &n);
+    const int rc = st.run(ctx, -1, &o, res, 64, &n);
     if (rc != B2DP_OK) {
-        logf("compute test at start not run: %s (%s)", b2dp_strerror(rc), b2dp_last_error(ctx));
+        logf("%s at start not run: %s (%s)", st.log, b2dp_strerror(rc), b2dp_last_error(ctx));
         return;
     }
     std::vector<b2dp_device> devs(n > 0 ? n : 1);
@@ -560,166 +569,12 @@ void run_compute_test(b2dp_ctx* ctx, const Flags& fl) {
     if (b2dp_enumerate(ctx, devs.data(), (int)devs.size(), &nd) != B2DP_OK) nd = 0;
     for (int i = 0; i < n; ++i) {
         const b2dp_compute_test_result& r = res[i];
-        logf("compute test %s: %s, flags 0x%x, SMs %d/%d, mismatches %llu/%llu/%llu, first bad SM %d, %.0f/%.0f/%.0f "
-             "TFLOP/s", r.device < nd ? devs[r.device].id : "?", r.healthy ? "Healthy" : "Unhealthy", r.flags,
-             r.sms_covered, r.sm_count, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
-             (unsigned long long)r.mismatches[2], r.first_bad_sm, r.tflops[0], r.tflops[1], r.tflops[2]);
-    }
-}
-
-// -fp_test_at_start=1: likewise for the FP32 / FP64 self-test (FFMA, DFMA, DMMA), after the compute test, for
-// -compute_test_ms per format.
-void run_fp_test(b2dp_ctx* ctx, const Flags& fl) {
-    b2dp_compute_test_opts o{};
-    o.duration_ms = fl.compute_test_ms;
-    o.fault_sm = -1;
-    if (fl.fp_test_at_start >= 2) o.flags |= B2DP_CT_EVEN_IF_BUSY;
-    b2dp_compute_test_result res[64];
-    int n = 0;
-    const int rc = b2dp_fp_test(ctx, -1, &o, res, 64, &n);
-    if (rc != B2DP_OK) {
-        logf("fp test at start not run: %s (%s)", b2dp_strerror(rc), b2dp_last_error(ctx));
-        return;
-    }
-    std::vector<b2dp_device> devs(n > 0 ? n : 1);
-    int nd = 0;
-    if (b2dp_enumerate(ctx, devs.data(), (int)devs.size(), &nd) != B2DP_OK) nd = 0;
-    for (int i = 0; i < n; ++i) {
-        const b2dp_compute_test_result& r = res[i];
-        logf("fp test %s: %s, flags 0x%x, SMs %d/%d, mismatches %llu/%llu/%llu, first bad SM %d, %.1f/%.1f/%.1f "
-             "TFLOP/s", r.device < nd ? devs[r.device].id : "?", r.healthy ? "Healthy" : "Unhealthy", r.flags,
-             r.sms_covered, r.sm_count, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
-             (unsigned long long)r.mismatches[2], r.first_bad_sm, r.tflops[0], r.tflops[1], r.tflops[2]);
-    }
-}
-
-// -sfu_test_at_start=1: likewise for the SFU self-test (MUFU transcendentals, checked against the SMs' majority and
-// host error bounds), after the FP test, for -compute_test_ms per format.
-void run_sfu_test(b2dp_ctx* ctx, const Flags& fl) {
-    b2dp_compute_test_opts o{};
-    o.duration_ms = fl.compute_test_ms;
-    o.fault_sm = -1;
-    if (fl.sfu_test_at_start >= 2) o.flags |= B2DP_CT_EVEN_IF_BUSY;
-    b2dp_compute_test_result res[64];
-    int n = 0;
-    const int rc = b2dp_sfu_test(ctx, -1, &o, res, 64, &n);
-    if (rc != B2DP_OK) {
-        logf("sfu test at start not run: %s (%s)", b2dp_strerror(rc), b2dp_last_error(ctx));
-        return;
-    }
-    std::vector<b2dp_device> devs(n > 0 ? n : 1);
-    int nd = 0;
-    if (b2dp_enumerate(ctx, devs.data(), (int)devs.size(), &nd) != B2DP_OK) nd = 0;
-    for (int i = 0; i < n; ++i) {
-        const b2dp_compute_test_result& r = res[i];
-        logf("sfu test %s: %s, flags 0x%x, SMs %d/%d, mismatches %llu/%llu/%llu, first bad SM %d, %.2f/%.2f/%.2f "
-             "T results/s", r.device < nd ? devs[r.device].id : "?", r.healthy ? "Healthy" : "Unhealthy", r.flags,
-             r.sms_covered, r.sm_count, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
-             (unsigned long long)r.mismatches[2], r.first_bad_sm, r.tflops[0], r.tflops[1], r.tflops[2]);
-    }
-}
-
-// -smem_test_at_start=1: likewise for the shared-memory self-test (every SM's 227 KiB array and the SM-to-SM DSMEM
-// path, marched against host patterns), after the SFU test, for -compute_test_ms per format.
-void run_smem_test(b2dp_ctx* ctx, const Flags& fl) {
-    b2dp_compute_test_opts o{};
-    o.duration_ms = fl.compute_test_ms;
-    o.fault_sm = -1;
-    if (fl.smem_test_at_start >= 2) o.flags |= B2DP_CT_EVEN_IF_BUSY;
-    b2dp_compute_test_result res[64];
-    int n = 0;
-    const int rc = b2dp_smem_test(ctx, -1, &o, res, 64, &n);
-    if (rc != B2DP_OK) {
-        logf("smem test at start not run: %s (%s)", b2dp_strerror(rc), b2dp_last_error(ctx));
-        return;
-    }
-    std::vector<b2dp_device> devs(n > 0 ? n : 1);
-    int nd = 0;
-    if (b2dp_enumerate(ctx, devs.data(), (int)devs.size(), &nd) != B2DP_OK) nd = 0;
-    for (int i = 0; i < n; ++i) {
-        const b2dp_compute_test_result& r = res[i];
-        logf("smem test %s: %s, flags 0x%x, SMs %d/%d, mismatches %llu/%llu/%llu, first bad SM %d, %.2f/%.2f/%.2f "
-             "TB/s", r.device < nd ? devs[r.device].id : "?", r.healthy ? "Healthy" : "Unhealthy", r.flags,
-             r.sms_covered, r.sm_count, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
-             (unsigned long long)r.mismatches[2], r.first_bad_sm, r.tflops[0], r.tflops[1], r.tflops[2]);
-    }
-}
-
-// -regfile_test_at_start=1: likewise for the register-file self-test (204 values per thread held in every SM's
-// registers and marched against host patterns), after the shared-memory test, for -compute_test_ms per format.
-void run_regfile_test(b2dp_ctx* ctx, const Flags& fl) {
-    b2dp_compute_test_opts o{};
-    o.duration_ms = fl.compute_test_ms;
-    o.fault_sm = -1;
-    if (fl.regfile_test_at_start >= 2) o.flags |= B2DP_CT_EVEN_IF_BUSY;
-    b2dp_compute_test_result res[64];
-    int n = 0;
-    const int rc = b2dp_regfile_test(ctx, -1, &o, res, 64, &n);
-    if (rc != B2DP_OK) {
-        logf("regfile test at start not run: %s (%s)", b2dp_strerror(rc), b2dp_last_error(ctx));
-        return;
-    }
-    std::vector<b2dp_device> devs(n > 0 ? n : 1);
-    int nd = 0;
-    if (b2dp_enumerate(ctx, devs.data(), (int)devs.size(), &nd) != B2DP_OK) nd = 0;
-    for (int i = 0; i < n; ++i) {
-        const b2dp_compute_test_result& r = res[i];
-        logf("regfile test %s: %s, flags 0x%x, SMs %d/%d, mismatches %llu/%llu/%llu, first bad SM %d, %.2f/%.2f/%.2f "
-             "TB/s", r.device < nd ? devs[r.device].id : "?", r.healthy ? "Healthy" : "Unhealthy", r.flags,
-             r.sms_covered, r.sm_count, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
-             (unsigned long long)r.mismatches[2], r.first_bad_sm, r.tflops[0], r.tflops[1], r.tflops[2]);
-    }
-}
-
-// -int_test_at_start=1: likewise for the integer and warp-exchange self-test (every SM's integer pipes and shuffle
-// network against exact host results), after the register-file test, for -compute_test_ms per format.
-void run_int_test(b2dp_ctx* ctx, const Flags& fl) {
-    b2dp_compute_test_opts o{};
-    o.duration_ms = fl.compute_test_ms;
-    o.fault_sm = -1;
-    if (fl.int_test_at_start >= 2) o.flags |= B2DP_CT_EVEN_IF_BUSY;
-    b2dp_compute_test_result res[64];
-    int n = 0;
-    const int rc = b2dp_int_test(ctx, -1, &o, res, 64, &n);
-    if (rc != B2DP_OK) {
-        logf("int test at start not run: %s (%s)", b2dp_strerror(rc), b2dp_last_error(ctx));
-        return;
-    }
-    std::vector<b2dp_device> devs(n > 0 ? n : 1);
-    int nd = 0;
-    if (b2dp_enumerate(ctx, devs.data(), (int)devs.size(), &nd) != B2DP_OK) nd = 0;
-    for (int i = 0; i < n; ++i) {
-        const b2dp_compute_test_result& r = res[i];
-        logf("int test %s: %s, flags 0x%x, SMs %d/%d, mismatches %llu/%llu/%llu, first bad SM %d, %.2f/%.2f/%.2f "
-             "T results/s", r.device < nd ? devs[r.device].id : "?", r.healthy ? "Healthy" : "Unhealthy", r.flags,
-             r.sms_covered, r.sm_count, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
-             (unsigned long long)r.mismatches[2], r.first_bad_sm, r.tflops[0], r.tflops[1], r.tflops[2]);
-    }
-}
-
-// -l2_test_at_start=1: likewise for the L2 self-test (a march over an L2-resident span that moves between SMs, and
-// the L2 atomic units, against host values), after the integer test, for -compute_test_ms per format.
-void run_l2_test(b2dp_ctx* ctx, const Flags& fl) {
-    b2dp_compute_test_opts o{};
-    o.duration_ms = fl.compute_test_ms;
-    o.fault_sm = -1;
-    if (fl.l2_test_at_start >= 2) o.flags |= B2DP_CT_EVEN_IF_BUSY;
-    b2dp_compute_test_result res[64];
-    int n = 0;
-    const int rc = b2dp_l2_test(ctx, -1, &o, res, 64, &n);
-    if (rc != B2DP_OK) {
-        logf("L2 test at start not run: %s (%s)", b2dp_strerror(rc), b2dp_last_error(ctx));
-        return;
-    }
-    std::vector<b2dp_device> devs(n > 0 ? n : 1);
-    int nd = 0;
-    if (b2dp_enumerate(ctx, devs.data(), (int)devs.size(), &nd) != B2DP_OK) nd = 0;
-    for (int i = 0; i < n; ++i) {
-        const b2dp_compute_test_result& r = res[i];
-        logf("L2 test %s: %s, flags 0x%x, SMs %d/%d, mismatches %llu/%llu/%llu, first bad SM %d, %.2f/%.2f/%.2f "
-             "TB/s, TB/s, G ops/s", r.device < nd ? devs[r.device].id : "?", r.healthy ? "Healthy" : "Unhealthy", r.flags,
-             r.sms_covered, r.sm_count, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
-             (unsigned long long)r.mismatches[2], r.first_bad_sm, r.tflops[0], r.tflops[1], r.tflops[2]);
+        char rate[96];
+        snprintf(rate, sizeof rate, st.rate, r.tflops[0], r.tflops[1], r.tflops[2]);
+        logf("%s %s: %s, flags 0x%x, SMs %d/%d, mismatches %llu/%llu/%llu, first bad SM %d, %s", st.log,
+             r.device < nd ? devs[r.device].id : "?", r.healthy ? "Healthy" : "Unhealthy", r.flags, r.sms_covered,
+             r.sm_count, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
+             (unsigned long long)r.mismatches[2], r.first_bad_sm, rate);
     }
 }
 
@@ -746,84 +601,6 @@ void run_hostlink_test(b2dp_ctx* ctx, const Flags& fl) {
              r.healthy ? "Healthy" : "Unhealthy", r.flags, (unsigned long long)r.mismatches[0],
              (unsigned long long)r.mismatches[1], (unsigned long long)r.mismatches[2], r.gbs[0], r.gbs[1], r.gbs[2],
              r.link_gen, r.link_width, (unsigned long long)r.replays);
-    }
-}
-
-// -half_test_at_start=1: likewise for the half-precision and conversion self-test (every SM's f16x2 / bf16x2 pipes and
-// type converters against exact host results), after the host-link test, for -compute_test_ms per format.
-void run_half_test(b2dp_ctx* ctx, const Flags& fl) {
-    b2dp_compute_test_opts o{};
-    o.duration_ms = fl.compute_test_ms;
-    o.fault_sm = -1;
-    if (fl.half_test_at_start >= 2) o.flags |= B2DP_CT_EVEN_IF_BUSY;
-    b2dp_compute_test_result res[64];
-    int n = 0;
-    const int rc = b2dp_half_test(ctx, -1, &o, res, 64, &n);
-    if (rc != B2DP_OK) {
-        logf("half test at start not run: %s (%s)", b2dp_strerror(rc), b2dp_last_error(ctx));
-        return;
-    }
-    std::vector<b2dp_device> devs(n > 0 ? n : 1);
-    int nd = 0;
-    if (b2dp_enumerate(ctx, devs.data(), (int)devs.size(), &nd) != B2DP_OK) nd = 0;
-    for (int i = 0; i < n; ++i) {
-        const b2dp_compute_test_result& r = res[i];
-        logf("half test %s: %s, flags 0x%x, SMs %d/%d, mismatches %llu/%llu/%llu, first bad SM %d, %.2f/%.2f/%.2f "
-             "T results/s", r.device < nd ? devs[r.device].id : "?", r.healthy ? "Healthy" : "Unhealthy", r.flags,
-             r.sms_covered, r.sm_count, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
-             (unsigned long long)r.mismatches[2], r.first_bad_sm, r.tflops[0], r.tflops[1], r.tflops[2]);
-    }
-}
-
-// -sync_test_at_start=1: likewise for the synchronization self-test (shared-memory atomics, barriers, mbarriers and
-// warp collectives against the PTX ISA), after the half-precision test, for -compute_test_ms per format.
-void run_sync_test(b2dp_ctx* ctx, const Flags& fl) {
-    b2dp_compute_test_opts o{};
-    o.duration_ms = fl.compute_test_ms;
-    o.fault_sm = -1;
-    if (fl.sync_test_at_start >= 2) o.flags |= B2DP_CT_EVEN_IF_BUSY;
-    b2dp_compute_test_result res[64];
-    int n = 0;
-    const int rc = b2dp_sync_test(ctx, -1, &o, res, 64, &n);
-    if (rc != B2DP_OK) {
-        logf("sync test at start not run: %s (%s)", b2dp_strerror(rc), b2dp_last_error(ctx));
-        return;
-    }
-    std::vector<b2dp_device> devs(n > 0 ? n : 1);
-    int nd = 0;
-    if (b2dp_enumerate(ctx, devs.data(), (int)devs.size(), &nd) != B2DP_OK) nd = 0;
-    for (int i = 0; i < n; ++i) {
-        const b2dp_compute_test_result& r = res[i];
-        logf("sync test %s: %s, flags 0x%x, SMs %d/%d, mismatches %llu/%llu/%llu, first bad SM %d, %.2f/%.2f/%.2f "
-             "G ops/s, G ops/s, T results/s", r.device < nd ? devs[r.device].id : "?", r.healthy ? "Healthy" : "Unhealthy", r.flags,
-             r.sms_covered, r.sm_count, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
-             (unsigned long long)r.mismatches[2], r.first_bad_sm, r.tflops[0], r.tflops[1], r.tflops[2]);
-    }
-}
-
-// -l1_test_at_start=1: likewise for the L1 self-test (the L1 data cache, the texture and read-only paths and the
-// constant cache against host-built data), after the synchronization test, for -compute_test_ms per format.
-void run_l1_test(b2dp_ctx* ctx, const Flags& fl) {
-    b2dp_compute_test_opts o{};
-    o.duration_ms = fl.compute_test_ms;
-    o.fault_sm = -1;
-    if (fl.l1_test_at_start >= 2) o.flags |= B2DP_CT_EVEN_IF_BUSY;
-    b2dp_compute_test_result res[64];
-    int n = 0;
-    const int rc = b2dp_l1_test(ctx, -1, &o, res, 64, &n);
-    if (rc != B2DP_OK) {
-        logf("L1 test at start not run: %s (%s)", b2dp_strerror(rc), b2dp_last_error(ctx));
-        return;
-    }
-    std::vector<b2dp_device> devs(n > 0 ? n : 1);
-    int nd = 0;
-    if (b2dp_enumerate(ctx, devs.data(), (int)devs.size(), &nd) != B2DP_OK) nd = 0;
-    for (int i = 0; i < n; ++i) {
-        const b2dp_compute_test_result& r = res[i];
-        logf("L1 test %s: %s, flags 0x%x, SMs %d/%d, mismatches %llu/%llu/%llu, first bad SM %d, %.2f/%.2f/%.2f "
-             "TB/s", r.device < nd ? devs[r.device].id : "?", r.healthy ? "Healthy" : "Unhealthy", r.flags,
-             r.sms_covered, r.sm_count, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
-             (unsigned long long)r.mismatches[2], r.first_bad_sm, r.tflops[0], r.tflops[1], r.tflops[2]);
     }
 }
 
@@ -858,17 +635,10 @@ int main(int argc, char** argv) {
     int rc = b2dp_open(fl.backend.c_str(), &ctx);
     if (rc != B2DP_OK) { logf("open %s: %s (%s)", fl.backend.c_str(), b2dp_strerror(rc), b2dp_last_error(nullptr)); return 1; }
     if (fl.memtest_at_start) run_memtest(ctx, fl);
-    if (fl.compute_test_at_start) run_compute_test(ctx, fl);
-    if (fl.fp_test_at_start) run_fp_test(ctx, fl);
-    if (fl.sfu_test_at_start) run_sfu_test(ctx, fl);
-    if (fl.smem_test_at_start) run_smem_test(ctx, fl);
-    if (fl.regfile_test_at_start) run_regfile_test(ctx, fl);
-    if (fl.int_test_at_start) run_int_test(ctx, fl);
-    if (fl.l2_test_at_start) run_l2_test(ctx, fl);
-    if (fl.hostlink_test_at_start) run_hostlink_test(ctx, fl);
-    if (fl.half_test_at_start) run_half_test(ctx, fl);
-    if (fl.sync_test_at_start) run_sync_test(ctx, fl);
-    if (fl.l1_test_at_start) run_l1_test(ctx, fl);
+    for (size_t t = 0; t < kNumSmTests; ++t) {
+        if (t == kSmTestsBeforeHostlink && fl.hostlink_test_at_start) run_hostlink_test(ctx, fl);
+        if (fl.sm_test_at_start[t]) run_sm_test(ctx, fl, t);
+    }
     char names[64][64];
     int n_res = 0;
     rc = b2dp_resource_list(ctx, fl.strategy.c_str(), names, 64, &n_res);  // main.go:141-146

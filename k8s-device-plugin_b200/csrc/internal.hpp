@@ -143,53 +143,32 @@ bool cuda_device_paths(CudaBackend*, const std::string& id, std::vector<std::str
 // xid=1: called (from a backend thread, or from b2dp_probe_inject_fault) when a device-level Xid has been latched
 void cuda_set_health_event_callback(CudaBackend*, std::function<void()> fn);
 
-// The on-demand diagnostics (the memory test and the compute and FP self-tests) are optional capabilities of the cuda backend:
-// a build of the library whose backend has none (the CPU-only build of ctx.cpp the sanitizer tests link against a
-// stand-in backend) simply leaves these null, and b2dp_memtest / b2dp_compute_test / b2dp_fp_test / b2dp_sfu_test /
-// b2dp_smem_test / b2dp_regfile_test / b2dp_int_test / b2dp_l2_test / b2dp_hostlink_test / b2dp_half_test /
-// b2dp_sync_test / b2dp_l1_test then return B2DP_E_UNSUPPORTED.
+// The ten on-demand SM self-tests, in the header's declaration order.  Each is one DiagSuite of cuda_backend.cu
+// (kSuites, indexed by this enum) behind one b2dp_<x>_test entry point of ctx.cpp.
+enum SmTest { SM_COMPUTE, SM_FP, SM_SFU, SM_SMEM, SM_REGFILE, SM_INT, SM_L2, SM_HALF, SM_SYNC, SM_L1, kSmTests };
+// the name each test goes by in its errors, per SmTest
+inline constexpr const char* kSmTestNames[kSmTests] = {
+    "compute self-test", "FP self-test", "SFU self-test", "shared-memory self-test", "register-file self-test",
+    "integer self-test", "L2 self-test", "half-precision self-test", "synchronization self-test", "L1 self-test"};
+
+// The on-demand diagnostics (the memory test, the SM self-tests and the host-link self-test) are optional capabilities
+// of the cuda backend: a build of the library whose backend has none (the CPU-only build of ctx.cpp the sanitizer tests
+// link against a stand-in backend) simply leaves these null, and b2dp_memtest, every b2dp_<x>_test and
+// b2dp_hostlink_test then return B2DP_E_UNSUPPORTED.
 // cuda_backend.cu fills them in during static initialisation.
 struct DiagHooks {
     // b2dp_memtest on `device` (-1 = all); B2DP_E_UNSUPPORTED without the in-process probe
     int (*memtest)(CudaBackend*, int device, const b2dp_memtest_opts* opts, std::vector<b2dp_memtest_result>& out,
                    std::string& err) = nullptr;
-    // b2dp_compute_test on `device` (-1 = all); B2DP_E_UNSUPPORTED without the in-process probe
-    int (*compute_test)(CudaBackend*, int device, const b2dp_compute_test_opts* opts,
-                        std::vector<b2dp_compute_test_result>& out, std::string& err) = nullptr;
-    // b2dp_fp_test on `device` (-1 = all); B2DP_E_UNSUPPORTED without the in-process probe
-    int (*fp_test)(CudaBackend*, int device, const b2dp_compute_test_opts* opts,
+    // the SM self-test `suite` (an SmTest) on `device` (-1 = all); B2DP_E_UNSUPPORTED without the in-process probe
+    int (*sm_test)(CudaBackend*, int suite, int device, const b2dp_compute_test_opts* opts,
                    std::vector<b2dp_compute_test_result>& out, std::string& err) = nullptr;
-    // true while any device carries a latched memtest, compute-test, FP-test, SFU-test, shared-memory-test,
-    // register-file-test, integer-test, L2-test, host-link-test or half-precision-test failure (cleared by
+    // true while any device carries a latched memtest, SM self-test or host-link self-test failure (cleared by
     // b2dp_probe_reset)
     bool (*latched)(CudaBackend*) = nullptr;
-    // b2dp_sfu_test on `device` (-1 = all); B2DP_E_UNSUPPORTED without the in-process probe
-    int (*sfu_test)(CudaBackend*, int device, const b2dp_compute_test_opts* opts,
-                    std::vector<b2dp_compute_test_result>& out, std::string& err) = nullptr;
-    // b2dp_smem_test on `device` (-1 = all); B2DP_E_UNSUPPORTED without the in-process probe
-    int (*smem_test)(CudaBackend*, int device, const b2dp_compute_test_opts* opts,
-                     std::vector<b2dp_compute_test_result>& out, std::string& err) = nullptr;
-    // b2dp_regfile_test on `device` (-1 = all); B2DP_E_UNSUPPORTED without the in-process probe
-    int (*regfile_test)(CudaBackend*, int device, const b2dp_compute_test_opts* opts,
-                        std::vector<b2dp_compute_test_result>& out, std::string& err) = nullptr;
-    // b2dp_int_test on `device` (-1 = all); B2DP_E_UNSUPPORTED without the in-process probe
-    int (*int_test)(CudaBackend*, int device, const b2dp_compute_test_opts* opts,
-                    std::vector<b2dp_compute_test_result>& out, std::string& err) = nullptr;
-    // b2dp_l2_test on `device` (-1 = all); B2DP_E_UNSUPPORTED without the in-process probe
-    int (*l2_test)(CudaBackend*, int device, const b2dp_compute_test_opts* opts,
-                   std::vector<b2dp_compute_test_result>& out, std::string& err) = nullptr;
     // b2dp_hostlink_test on `device` (-1 = all); B2DP_E_UNSUPPORTED without the in-process probe
     int (*hostlink_test)(CudaBackend*, int device, const b2dp_hostlink_opts* opts,
                          std::vector<b2dp_hostlink_result>& out, std::string& err) = nullptr;
-    // b2dp_half_test on `device` (-1 = all); B2DP_E_UNSUPPORTED without the in-process probe
-    int (*half_test)(CudaBackend*, int device, const b2dp_compute_test_opts* opts,
-                     std::vector<b2dp_compute_test_result>& out, std::string& err) = nullptr;
-    // b2dp_sync_test on `device` (-1 = all); B2DP_E_UNSUPPORTED without the in-process probe
-    int (*sync_test)(CudaBackend*, int device, const b2dp_compute_test_opts* opts,
-                     std::vector<b2dp_compute_test_result>& out, std::string& err) = nullptr;
-    // b2dp_l1_test on `device` (-1 = all); B2DP_E_UNSUPPORTED without the in-process probe
-    int (*l1_test)(CudaBackend*, int device, const b2dp_compute_test_opts* opts,
-                   std::vector<b2dp_compute_test_result>& out, std::string& err) = nullptr;
 };
 DiagHooks& diag_hooks();  // ctx.cpp
 

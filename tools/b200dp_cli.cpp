@@ -31,6 +31,31 @@ static int die(b2dp_ctx* c, const char* what, int rc) {
     fprintf(stderr, "%s: %s [%d] %s\n", what, b2dp_strerror(rc), rc, c ? b2dp_last_error(c) : "");
     return 1;
 }
+// The SM self-test commands: all ten take b2dp_compute_test_opts and print b2dp_compute_test_result the same way, up
+// to the names and precision of the rate columns.
+struct SmTestCmd {
+    const char* cmd;
+    int (*run)(b2dp_ctx*, int, const b2dp_compute_test_opts*, b2dp_compute_test_result*, int, int*);
+    const char* label;  // the entry point, in an error
+    const char* rates;  // tflops[0..2]
+};
+static constexpr SmTestCmd kSmTestCmds[] = {
+    {"compute_test", b2dp_compute_test, "b2dp_compute_test", "tflops_bf16=%.0f tflops_fp8=%.0f tops_int8=%.0f"},
+    {"fp_test", b2dp_fp_test, "b2dp_fp_test", "tflops_fp32=%.1f tflops_fp64=%.1f tflops_dmma=%.1f"},
+    {"sfu_test", b2dp_sfu_test, "b2dp_sfu_test", "tresults_f32=%.2f tresults_root=%.2f tresults_f16=%.2f"},
+    {"smem_test", b2dp_smem_test, "b2dp_smem_test", "tbs_word=%.2f tbs_byte=%.2f tbs_dsmem=%.2f"},
+    {"regfile_test", b2dp_regfile_test, "b2dp_regfile_test", "tbs_alu=%.2f tbs_load=%.2f tbs_hold=%.2f"},
+    {"int_test", b2dp_int_test, "b2dp_int_test", "tresults_mad=%.2f tresults_bit=%.2f tresults_warp=%.2f"},
+    {"l2_test", b2dp_l2_test, "b2dp_l2_test", "tbs_word=%.2f tbs_byte=%.2f gops_atom=%.2f"},
+    {"half_test", b2dp_half_test, "b2dp_half_test", "tresults_f16=%.2f tresults_bf16=%.2f tresults_cvt=%.2f"},
+    {"sync_test", b2dp_sync_test, "b2dp_sync_test", "gops_atom=%.2f gops_bar=%.2f tresults_warp=%.2f"},
+    {"l1_test", b2dp_l1_test, "b2dp_l1_test", "tbs_data=%.2f tbs_tex=%.2f tbs_const=%.2f"},
+};
+static const SmTestCmd* find_sm_test(const std::string& cmd) {
+    for (const SmTestCmd& t : kSmTestCmds)
+        if (cmd == t.cmd) return &t;
+    return nullptr;
+}
 static double median(std::vector<double> v) { std::sort(v.begin(), v.end()); return v.empty() ? 0 : v[v.size() / 2]; }
 static double pct(std::vector<double> v, double q) {
     std::sort(v.begin(), v.end());
@@ -156,217 +181,24 @@ int main(int argc, char** argv) {
         }
         b2dp_close(ctx);
         return bad ? 1 : 0;
-    } else if (cmd == "compute_test") {  // one line per device; exit status 1 if any device is Unhealthy
+    } else if (const SmTestCmd* t = find_sm_test(cmd)) {  // one line per device; exit status 1 if any device is Unhealthy
         b2dp_compute_test_opts co{};
         co.duration_ms = argc > 3 ? (uint32_t)strtoul(argv[3], nullptr, 0) : 0;
         co.fault_sm = -1;
         std::vector<b2dp_compute_test_result> res(n ? n : 1);
         int m = 0;
-        if ((rc = b2dp_compute_test(ctx, -1, &co, res.data(), (int)res.size(), &m)) != B2DP_OK)
-            return die(ctx, "b2dp_compute_test", rc);
+        if ((rc = t->run(ctx, -1, &co, res.data(), (int)res.size(), &m)) != B2DP_OK) return die(ctx, t->label, rc);
         int bad = 0;
         for (int i = 0; i < m; ++i) {
             const b2dp_compute_test_result& r = res[i];
             printf("%s %s err=%d flags=0x%x sms=%d/%d nsmid=%d mismatches=%llu,%llu,%llu first_bad_sm=%d "
-                   "first_bad_format=%d first_bad_tile=%d ms=%.1f,%.1f,%.1f tflops_bf16=%.0f tflops_fp8=%.0f tops_int8=%.0f\n",
+                   "first_bad_format=%d first_bad_tile=%d ms=%.1f,%.1f,%.1f ",
                    devs[r.device].id, r.healthy ? "Healthy" : "Unhealthy", r.err, r.flags, r.sms_covered, r.sm_count,
                    r.nsmid, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
                    (unsigned long long)r.mismatches[2], r.first_bad_sm, r.first_bad_format, r.first_bad_tile, r.ms[0],
-                   r.ms[1], r.ms[2], r.tflops[0], r.tflops[1], r.tflops[2]);
-            bad += !r.healthy;
-        }
-        b2dp_close(ctx);
-        return bad ? 1 : 0;
-    } else if (cmd == "fp_test") {  // one line per device; exit status 1 if any device is Unhealthy
-        b2dp_compute_test_opts co{};
-        co.duration_ms = argc > 3 ? (uint32_t)strtoul(argv[3], nullptr, 0) : 0;
-        co.fault_sm = -1;
-        std::vector<b2dp_compute_test_result> res(n ? n : 1);
-        int m = 0;
-        if ((rc = b2dp_fp_test(ctx, -1, &co, res.data(), (int)res.size(), &m)) != B2DP_OK) return die(ctx, "b2dp_fp_test", rc);
-        int bad = 0;
-        for (int i = 0; i < m; ++i) {
-            const b2dp_compute_test_result& r = res[i];
-            printf("%s %s err=%d flags=0x%x sms=%d/%d nsmid=%d mismatches=%llu,%llu,%llu first_bad_sm=%d "
-                   "first_bad_format=%d first_bad_tile=%d ms=%.1f,%.1f,%.1f tflops_fp32=%.1f tflops_fp64=%.1f tflops_dmma=%.1f\n",
-                   devs[r.device].id, r.healthy ? "Healthy" : "Unhealthy", r.err, r.flags, r.sms_covered, r.sm_count,
-                   r.nsmid, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
-                   (unsigned long long)r.mismatches[2], r.first_bad_sm, r.first_bad_format, r.first_bad_tile, r.ms[0],
-                   r.ms[1], r.ms[2], r.tflops[0], r.tflops[1], r.tflops[2]);
-            bad += !r.healthy;
-        }
-        b2dp_close(ctx);
-        return bad ? 1 : 0;
-    } else if (cmd == "sfu_test") {  // one line per device; exit status 1 if any device is Unhealthy
-        b2dp_compute_test_opts co{};
-        co.duration_ms = argc > 3 ? (uint32_t)strtoul(argv[3], nullptr, 0) : 0;
-        co.fault_sm = -1;
-        std::vector<b2dp_compute_test_result> res(n ? n : 1);
-        int m = 0;
-        if ((rc = b2dp_sfu_test(ctx, -1, &co, res.data(), (int)res.size(), &m)) != B2DP_OK) return die(ctx, "b2dp_sfu_test", rc);
-        int bad = 0;
-        for (int i = 0; i < m; ++i) {
-            const b2dp_compute_test_result& r = res[i];
-            printf("%s %s err=%d flags=0x%x sms=%d/%d nsmid=%d mismatches=%llu,%llu,%llu first_bad_sm=%d "
-                   "first_bad_format=%d first_bad_tile=%d ms=%.1f,%.1f,%.1f tresults_f32=%.2f tresults_root=%.2f "
-                   "tresults_f16=%.2f\n",
-                   devs[r.device].id, r.healthy ? "Healthy" : "Unhealthy", r.err, r.flags, r.sms_covered, r.sm_count,
-                   r.nsmid, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
-                   (unsigned long long)r.mismatches[2], r.first_bad_sm, r.first_bad_format, r.first_bad_tile, r.ms[0],
-                   r.ms[1], r.ms[2], r.tflops[0], r.tflops[1], r.tflops[2]);
-            bad += !r.healthy;
-        }
-        b2dp_close(ctx);
-        return bad ? 1 : 0;
-    } else if (cmd == "smem_test") {  // one line per device; exit status 1 if any device is Unhealthy
-        b2dp_compute_test_opts co{};
-        co.duration_ms = argc > 3 ? (uint32_t)strtoul(argv[3], nullptr, 0) : 0;
-        co.fault_sm = -1;
-        std::vector<b2dp_compute_test_result> res(n ? n : 1);
-        int m = 0;
-        if ((rc = b2dp_smem_test(ctx, -1, &co, res.data(), (int)res.size(), &m)) != B2DP_OK) return die(ctx, "b2dp_smem_test", rc);
-        int bad = 0;
-        for (int i = 0; i < m; ++i) {
-            const b2dp_compute_test_result& r = res[i];
-            printf("%s %s err=%d flags=0x%x sms=%d/%d nsmid=%d mismatches=%llu,%llu,%llu first_bad_sm=%d "
-                   "first_bad_format=%d first_bad_tile=%d ms=%.1f,%.1f,%.1f tbs_word=%.2f tbs_byte=%.2f "
-                   "tbs_dsmem=%.2f\n",
-                   devs[r.device].id, r.healthy ? "Healthy" : "Unhealthy", r.err, r.flags, r.sms_covered, r.sm_count,
-                   r.nsmid, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
-                   (unsigned long long)r.mismatches[2], r.first_bad_sm, r.first_bad_format, r.first_bad_tile, r.ms[0],
-                   r.ms[1], r.ms[2], r.tflops[0], r.tflops[1], r.tflops[2]);
-            bad += !r.healthy;
-        }
-        b2dp_close(ctx);
-        return bad ? 1 : 0;
-    } else if (cmd == "regfile_test") {  // one line per device; exit status 1 if any device is Unhealthy
-        b2dp_compute_test_opts co{};
-        co.duration_ms = argc > 3 ? (uint32_t)strtoul(argv[3], nullptr, 0) : 0;
-        co.fault_sm = -1;
-        std::vector<b2dp_compute_test_result> res(n ? n : 1);
-        int m = 0;
-        if ((rc = b2dp_regfile_test(ctx, -1, &co, res.data(), (int)res.size(), &m)) != B2DP_OK)
-            return die(ctx, "b2dp_regfile_test", rc);
-        int bad = 0;
-        for (int i = 0; i < m; ++i) {
-            const b2dp_compute_test_result& r = res[i];
-            printf("%s %s err=%d flags=0x%x sms=%d/%d nsmid=%d mismatches=%llu,%llu,%llu first_bad_sm=%d "
-                   "first_bad_format=%d first_bad_tile=%d ms=%.1f,%.1f,%.1f tbs_alu=%.2f tbs_load=%.2f "
-                   "tbs_hold=%.2f\n",
-                   devs[r.device].id, r.healthy ? "Healthy" : "Unhealthy", r.err, r.flags, r.sms_covered, r.sm_count,
-                   r.nsmid, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
-                   (unsigned long long)r.mismatches[2], r.first_bad_sm, r.first_bad_format, r.first_bad_tile, r.ms[0],
-                   r.ms[1], r.ms[2], r.tflops[0], r.tflops[1], r.tflops[2]);
-            bad += !r.healthy;
-        }
-        b2dp_close(ctx);
-        return bad ? 1 : 0;
-    } else if (cmd == "int_test") {  // one line per device; exit status 1 if any device is Unhealthy
-        b2dp_compute_test_opts co{};
-        co.duration_ms = argc > 3 ? (uint32_t)strtoul(argv[3], nullptr, 0) : 0;
-        co.fault_sm = -1;
-        std::vector<b2dp_compute_test_result> res(n ? n : 1);
-        int m = 0;
-        if ((rc = b2dp_int_test(ctx, -1, &co, res.data(), (int)res.size(), &m)) != B2DP_OK)
-            return die(ctx, "b2dp_int_test", rc);
-        int bad = 0;
-        for (int i = 0; i < m; ++i) {
-            const b2dp_compute_test_result& r = res[i];
-            printf("%s %s err=%d flags=0x%x sms=%d/%d nsmid=%d mismatches=%llu,%llu,%llu first_bad_sm=%d "
-                   "first_bad_format=%d first_bad_tile=%d ms=%.1f,%.1f,%.1f tresults_mad=%.2f "
-                   "tresults_bit=%.2f tresults_warp=%.2f\n",
-                   devs[r.device].id, r.healthy ? "Healthy" : "Unhealthy", r.err, r.flags, r.sms_covered, r.sm_count,
-                   r.nsmid, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
-                   (unsigned long long)r.mismatches[2], r.first_bad_sm, r.first_bad_format, r.first_bad_tile, r.ms[0],
-                   r.ms[1], r.ms[2], r.tflops[0], r.tflops[1], r.tflops[2]);
-            bad += !r.healthy;
-        }
-        b2dp_close(ctx);
-        return bad ? 1 : 0;
-    } else if (cmd == "l2_test") {  // one line per device; exit status 1 if any device is Unhealthy
-        b2dp_compute_test_opts co{};
-        co.duration_ms = argc > 3 ? (uint32_t)strtoul(argv[3], nullptr, 0) : 0;
-        co.fault_sm = -1;
-        std::vector<b2dp_compute_test_result> res(n ? n : 1);
-        int m = 0;
-        if ((rc = b2dp_l2_test(ctx, -1, &co, res.data(), (int)res.size(), &m)) != B2DP_OK)
-            return die(ctx, "b2dp_l2_test", rc);
-        int bad = 0;
-        for (int i = 0; i < m; ++i) {
-            const b2dp_compute_test_result& r = res[i];
-            printf("%s %s err=%d flags=0x%x sms=%d/%d nsmid=%d mismatches=%llu,%llu,%llu first_bad_sm=%d "
-                   "first_bad_format=%d first_bad_tile=%d ms=%.1f,%.1f,%.1f tbs_word=%.2f "
-                   "tbs_byte=%.2f gops_atom=%.2f\n",
-                   devs[r.device].id, r.healthy ? "Healthy" : "Unhealthy", r.err, r.flags, r.sms_covered, r.sm_count,
-                   r.nsmid, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
-                   (unsigned long long)r.mismatches[2], r.first_bad_sm, r.first_bad_format, r.first_bad_tile, r.ms[0],
-                   r.ms[1], r.ms[2], r.tflops[0], r.tflops[1], r.tflops[2]);
-            bad += !r.healthy;
-        }
-        b2dp_close(ctx);
-        return bad ? 1 : 0;
-    } else if (cmd == "half_test") {  // one line per device; exit status 1 if any device is Unhealthy
-        b2dp_compute_test_opts co{};
-        co.duration_ms = argc > 3 ? (uint32_t)strtoul(argv[3], nullptr, 0) : 0;
-        co.fault_sm = -1;
-        std::vector<b2dp_compute_test_result> res(n ? n : 1);
-        int m = 0;
-        if ((rc = b2dp_half_test(ctx, -1, &co, res.data(), (int)res.size(), &m)) != B2DP_OK)
-            return die(ctx, "b2dp_half_test", rc);
-        int bad = 0;
-        for (int i = 0; i < m; ++i) {
-            const b2dp_compute_test_result& r = res[i];
-            printf("%s %s err=%d flags=0x%x sms=%d/%d nsmid=%d mismatches=%llu,%llu,%llu first_bad_sm=%d "
-                   "first_bad_format=%d first_bad_tile=%d ms=%.1f,%.1f,%.1f tresults_f16=%.2f "
-                   "tresults_bf16=%.2f tresults_cvt=%.2f\n",
-                   devs[r.device].id, r.healthy ? "Healthy" : "Unhealthy", r.err, r.flags, r.sms_covered, r.sm_count,
-                   r.nsmid, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
-                   (unsigned long long)r.mismatches[2], r.first_bad_sm, r.first_bad_format, r.first_bad_tile, r.ms[0],
-                   r.ms[1], r.ms[2], r.tflops[0], r.tflops[1], r.tflops[2]);
-            bad += !r.healthy;
-        }
-        b2dp_close(ctx);
-        return bad ? 1 : 0;
-    } else if (cmd == "sync_test") {  // one line per device; exit status 1 if any device is Unhealthy
-        b2dp_compute_test_opts co{};
-        co.duration_ms = argc > 3 ? (uint32_t)strtoul(argv[3], nullptr, 0) : 0;
-        co.fault_sm = -1;
-        std::vector<b2dp_compute_test_result> res(n ? n : 1);
-        int m = 0;
-        if ((rc = b2dp_sync_test(ctx, -1, &co, res.data(), (int)res.size(), &m)) != B2DP_OK)
-            return die(ctx, "b2dp_sync_test", rc);
-        int bad = 0;
-        for (int i = 0; i < m; ++i) {
-            const b2dp_compute_test_result& r = res[i];
-            printf("%s %s err=%d flags=0x%x sms=%d/%d nsmid=%d mismatches=%llu,%llu,%llu first_bad_sm=%d "
-                   "first_bad_format=%d first_bad_tile=%d ms=%.1f,%.1f,%.1f gops_atom=%.2f "
-                   "gops_bar=%.2f tresults_warp=%.2f\n",
-                   devs[r.device].id, r.healthy ? "Healthy" : "Unhealthy", r.err, r.flags, r.sms_covered, r.sm_count,
-                   r.nsmid, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
-                   (unsigned long long)r.mismatches[2], r.first_bad_sm, r.first_bad_format, r.first_bad_tile, r.ms[0],
-                   r.ms[1], r.ms[2], r.tflops[0], r.tflops[1], r.tflops[2]);
-            bad += !r.healthy;
-        }
-        b2dp_close(ctx);
-        return bad ? 1 : 0;
-    } else if (cmd == "l1_test") {  // one line per device; exit status 1 if any device is Unhealthy
-        b2dp_compute_test_opts co{};
-        co.duration_ms = argc > 3 ? (uint32_t)strtoul(argv[3], nullptr, 0) : 0;
-        co.fault_sm = -1;
-        std::vector<b2dp_compute_test_result> res(n ? n : 1);
-        int m = 0;
-        if ((rc = b2dp_l1_test(ctx, -1, &co, res.data(), (int)res.size(), &m)) != B2DP_OK)
-            return die(ctx, "b2dp_l1_test", rc);
-        int bad = 0;
-        for (int i = 0; i < m; ++i) {
-            const b2dp_compute_test_result& r = res[i];
-            printf("%s %s err=%d flags=0x%x sms=%d/%d nsmid=%d mismatches=%llu,%llu,%llu first_bad_sm=%d "
-                   "first_bad_format=%d first_bad_tile=%d ms=%.1f,%.1f,%.1f tbs_data=%.2f "
-                   "tbs_tex=%.2f tbs_const=%.2f\n",
-                   devs[r.device].id, r.healthy ? "Healthy" : "Unhealthy", r.err, r.flags, r.sms_covered, r.sm_count,
-                   r.nsmid, (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
-                   (unsigned long long)r.mismatches[2], r.first_bad_sm, r.first_bad_format, r.first_bad_tile, r.ms[0],
-                   r.ms[1], r.ms[2], r.tflops[0], r.tflops[1], r.tflops[2]);
+                   r.ms[1], r.ms[2]);
+            printf(t->rates, r.tflops[0], r.tflops[1], r.tflops[2]);
+            printf("\n");
             bad += !r.healthy;
         }
         b2dp_close(ctx);
