@@ -184,6 +184,16 @@ typedef struct b2dp_ctx b2dp_ctx;
  *                     pass is armed, its stream wait stalls all other GPU work THIS PROCESS submits to that GPU (other streams,
  *                     a second context of this library; measured) -- other processes are not affected (a tenant's kernels
  *                     keep their latency).  Use it only where the library is the process's sole user of the GPU (the daemon).
+ *                     sm_check=<ms, 0..10000, default 0 = off>: every probe pass (b2dp_probe_health, every heartbeat)
+ *                     also runs one of the ten SM self-tests, in rotation, on every GPU whose HBM pass completed in that
+ *                     call and that no other process uses (NVML), for <ms> per format, after the HBM pass (whose fields
+ *                     it does not change).  Each GPU moves to the next test only when it ran one, so an idle GPU runs
+ *                     all ten every ten passes.  The pass reports it with B2DP_RES_SM_CHECK and the sm_check field; a
+ *                     failure or timeout latches B2DP_RES_COMPUTE in the same result, exactly as the on-demand tests
+ *                     do.  prearm=1 does not arm while it is on.  In-process probe only: with probe=helpers,
+ *                     probe=off or MIG the key is accepted, logged as off and ignored.
+ *                     sm_check_fault=<smid>+<mask> (test hook): every SM check flips `mask` in one result on the SM
+ *                     with that %smid, as b2dp_compute_test_opts.fault_sm / fault_mask do.
  *                     seed_index=<i>: (helpers) the enumeration index this one-device context stands for.
  *                     A GPU whose own setup fails (or that break=<i>+<j>, a test hook, names by enumeration index)
  *                     stays in the device list and is reported Unhealthy with B2DP_E_CUDA on every pass; the open
@@ -251,7 +261,9 @@ typedef struct b2dp_probe_result {
     float frac;                 /* (bytes / ms_device) / gbs_ref: the verdict's rate over the ceiling, both on the in-kernel
                                    clock (0 if there is no ceiling) */
     float min_gbs_applied;      /* the floor the verdict used: min_gbs, else min_frac x gbs_ref, else 0 (none) */
-    uint32_t reserved;
+    uint32_t sm_check;          /* sm_check=: 1 + the SM self-test this pass ran after its HBM pass, in this header's
+                                   order (1 compute, 2 FP, 3 SFU, 4 shared memory, 5 register file, 6 integer, 7 L2,
+                                   8 half precision, 9 synchronization, 10 L1); 0 if none ran (B2DP_RES_SM_CHECK) */
 } b2dp_probe_result;
 #define B2DP_RES_SKIPPED_BUSY 0x1u /* busy=skip: another process owns the GPU, no pass ran, the last verdict stands */
 #define B2DP_RES_SHRUNK 0x2u       /* busy=shrink: a prefix (shrink_bytes) was verified without re-keying; no GB/s floor */
@@ -273,11 +285,13 @@ typedef struct b2dp_probe_result {
 #define B2DP_RES_COMPUTE 0x400u    /* a compute, FP, SFU, shared-memory, register-file, integer, L2, half-precision,
                                       synchronization or L1 self-test (b2dp_compute_test, b2dp_fp_test, b2dp_sfu_test,
                                       b2dp_smem_test, b2dp_regfile_test, b2dp_int_test, b2dp_l2_test, b2dp_half_test,
-                                      b2dp_sync_test, b2dp_l1_test) of this device
-                                      failed or timed out since open (or the last b2dp_probe_reset) => Unhealthy,
-                                      sticky */
+                                      b2dp_sync_test, b2dp_l1_test) of this device, or a heartbeat's SM check
+                                      (sm_check=), failed or timed out since open (or the last b2dp_probe_reset)
+                                      => Unhealthy, sticky */
 #define B2DP_RES_HOSTLINK 0x800u   /* a b2dp_hostlink_test of this device failed or timed out since open (or the last
                                       b2dp_probe_reset) => Unhealthy, sticky */
+#define B2DP_RES_SM_CHECK 0x1000u  /* sm_check=: this pass also ran one SM self-test slice on this device, after its HBM
+                                      pass (which one: the sm_check field); a failed slice also sets B2DP_RES_COMPUTE */
 
 /* Replaces the exporter round trip getGPUHealth (exporter/health.go:42-82) and the evidence behind simpleHealthCheck
  * (plugin.go:161-206): launch the probe on every GPU of the context concurrently (one worker thread + stream per
@@ -713,7 +727,7 @@ typedef struct b2dp_cycle_stats {
     int32_t node_healthy;     /* simpleHealthCheck result (heartbeat) */
     float ms_total;           /* wall clock of the call */
     float ms_enumerate;
-    float ms_probe;           /* launch-all .. last result */
+    float ms_probe;           /* launch-all .. last result, including the SM check slices of sm_check= */
     float ms_encode;
     float probe_gbs_min;      /* over devices, 0 if no probe ran */
     float probe_gbs_sum;

@@ -57,6 +57,7 @@ L1_DATA, L1_TEX, L1_CONST = 0, 1, 2
 L2_WORD, L2_BYTE, L2_ATOM = 0, 1, 2
 CT_ECC_CORRECTED, CT_ECC, CT_NO_ECC = 0x10, 0x20, 0x40
 RES_HOSTLINK = 0x800
+RES_SM_CHECK = 0x1000
 HL_EVEN_IF_BUSY = 1
 HL_H2D, HL_D2H, HL_SM = 0, 1, 2
 HL_SKIPPED_BUSY, HL_NUMA_UNBOUND, HL_LINK_NARROW, HL_LINK_SLOW, HL_REPLAYS, HL_NO_NVML = 1, 2, 4, 8, 0x10, 0x20
@@ -103,7 +104,7 @@ class ProbeResult(C.Structure):
                 ("checksum", C.c_uint64), ("expected_checksum", C.c_uint64), ("mismatches", C.c_uint64),
                 ("first_bad_word", C.c_uint64), ("bytes", C.c_uint64), ("ms_event", C.c_float),
                 ("ms_device", C.c_float), ("gbs", C.c_float), ("flags", C.c_uint32), ("gbs_ref", C.c_float),
-                ("frac", C.c_float), ("min_gbs_applied", C.c_float), ("reserved", C.c_uint32)]
+                ("frac", C.c_float), ("min_gbs_applied", C.c_float), ("sm_check", C.c_uint32)]
 
 
 class CycleOpts(C.Structure):

@@ -25,6 +25,7 @@ class ProbeResult:
     gbs_ref: float = 0.0           # the device's calibrated ceiling
     frac: float = 0.0              # gbs / gbs_ref
     min_gbs_applied: float = 0.0   # the floor the verdict used
+    sm_check: int = 0              # sm_check=: 1 + the SM self-test this pass ran (1 compute .. 10 L1), 0 if none
 
 
 @dataclass
@@ -200,7 +201,7 @@ class Context:
         N.check(rc, self._h)
         return [ProbeResult(r.device, bool(r.healthy), r.err, r.seed, r.checksum, r.expected_checksum, r.mismatches,
                             r.first_bad_word, r.bytes, r.ms_event, r.ms_device, r.gbs, r.flags, r.gbs_ref, r.frac,
-                            r.min_gbs_applied) for r in arr[:n]]
+                            r.min_gbs_applied, r.sm_check) for r in arr[:n]]
 
     def probe_inject_fault(self, device: int, word_index: int, mask: int):
         N.check(N.lib.b2dp_probe_inject_fault(self._h, device, word_index, mask), self._h)

@@ -149,6 +149,25 @@ static bool parse_kv(const std::string& body, std::map<std::string, std::string>
     return true;
 }
 
+// A whole number in [0, max]: decimal digits only, or 0x and hex digits when `hex`; no sign, no blanks, no suffix.
+static bool parse_uint(const std::string& s, uint64_t max, bool hex, uint64_t* out) {
+    const bool is_hex = hex && s.size() > 2 && s[0] == '0' && (s[1] == 'x' || s[1] == 'X');
+    const std::string digits = is_hex ? s.substr(2) : s;
+    if (digits.empty() || digits.size() > 16) return false;
+    uint64_t v = 0;
+    for (char ch : digits) {
+        int d;
+        if (ch >= '0' && ch <= '9') d = ch - '0';
+        else if (is_hex && ch >= 'a' && ch <= 'f') d = ch - 'a' + 10;
+        else if (is_hex && ch >= 'A' && ch <= 'F') d = ch - 'A' + 10;
+        else return false;
+        v = v * (is_hex ? 16 : 10) + (uint64_t)d;
+        if (v > max) return false;
+    }
+    *out = v;
+    return true;
+}
+
 extern "C" int b2dp_open(const char* uri, b2dp_ctx** out) {
     if (!uri || !out) return B2DP_E_INVAL;
     *out = nullptr;
@@ -260,6 +279,18 @@ extern "C" int b2dp_open(const char* uri, b2dp_ctx** out) {
                     if (e > pos) cfg.break_devices.push_back(atoi(p.second.substr(pos, e - pos).c_str()));
                     pos = e + 1;
                 }
+            } else if (p.first == "sm_check") {
+                uint64_t ms = 0;
+                if (!parse_uint(p.second, 10000, false, &ms)) return fail(B2DP_E_INVAL, "sm_check= wants a whole number of ms in [0, 10000]");
+                cfg.sm_check_ms = (uint32_t)ms;
+            } else if (p.first == "sm_check_fault") {
+                const size_t plus = p.second.find('+');
+                uint64_t sm = 0, mask = 0;
+                if (plus == std::string::npos || !parse_uint(p.second.substr(0, plus), 255, false, &sm) ||
+                    !parse_uint(p.second.substr(plus + 1), 0xffffffffull, true, &mask))
+                    return fail(B2DP_E_INVAL, "sm_check_fault= wants <smid>+<mask>, an SM id in [0, 255] and a 32-bit mask");
+                cfg.sm_check_fault_sm = (int)sm;
+                cfg.sm_check_fault_mask = (uint32_t)mask;
             }
             else return fail(B2DP_E_INVAL, "unknown cuda: option " + p.first);
         }

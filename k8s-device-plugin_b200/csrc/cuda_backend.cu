@@ -120,6 +120,7 @@ struct Gpu {
     std::atomic<bool> memtest_fault{false};        // a b2dp_memtest failed or timed out (sticky until b2dp_probe_reset)
     std::atomic<bool> compute_fault{false};        // a b2dp_compute_test or b2dp_fp_test failed or timed out (likewise)
     std::atomic<bool> hostlink_fault{false};       // a b2dp_hostlink_test failed or timed out (likewise)
+    int sm_check_next = 0;                         // sm_check=: the SmTest this GPU's next slice runs (under probe_mu)
     int last_healthy = 1;
     // worker
     std::thread th;
@@ -439,6 +440,11 @@ int cuda_backend_open(const CudaConfig& cfg, CudaBackend** out, std::string& err
             logf(0, "NVML enumeration: %zu unit(s), %d MIG instance(s), probe=%s%s", be->units->units.size(), n_mig, mode == 1 ? "helpers" : "off",
                  cfg.probe_mode == 0 ? " (forced by MIG: CUDA shows a process one compute instance)" : "");
         }
+        if (cfg.sm_check_ms)  // the SM self-tests run in the in-process probe only
+            logf(1, "SM checks are off (sm_check=%u): %s", cfg.sm_check_ms,
+                 mode == 2 ? "probe=off runs no probe pass"
+                 : cfg.probe_mode == 0 ? "MIG forces probe=helpers, and they run in the in-process probe only"
+                                       : "they run in the in-process probe only, not in probe=helpers children");
         if (be->nvml.driver_version) {
             char buf[96] = {0};
             if (be->nvml.driver_version(buf, sizeof buf) == 0) be->driver_version = buf;
@@ -887,6 +893,8 @@ static void xid_listener(CudaBackend* be) {
     }
 }
 
+static void sm_check_slices(CudaBackend* be, const std::vector<char>& ran, std::vector<b2dp_probe_result>& out);
+
 int cuda_probe(CudaBackend* be, const b2dp_probe_opts* opts, std::vector<b2dp_probe_result>& out, std::string& err) {
     std::lock_guard<std::mutex> pl(be->probe_mu);
     if (be->units) {
@@ -972,7 +980,9 @@ int cuda_probe(CudaBackend* be, const b2dp_probe_opts* opts, std::vector<b2dp_pr
             if (L->sleeping.load()) { std::lock_guard<std::mutex> l(L->mu); L->cv.notify_one(); }
         }
         // prearm=1: a pass with the default options may be the one that is already enqueued behind its doorbell
-        const bool can_arm = be->wait32 && variant == B2DP_PROBE_VARIANT_TMA && !timed && grid == 0 && be->cfg.busy_policy == 0;
+        // (not with sm_check=: the slice after every pass would flush the armed one)
+        const bool can_arm = be->wait32 && variant == B2DP_PROBE_VARIANT_TMA && !timed && grid == 0 &&
+                             be->cfg.busy_policy == 0 && be->cfg.sm_check_ms == 0;
         std::vector<char> arm_ok(n, 0);  // decided before any pass is issued (issuing fills in r->n_vec)
         for (size_t i = 0; i < n; ++i) arm_ok[i] = can_arm && res[i]->n_vec == 0 && res[i]->advance;
         auto armable = [&](size_t i) { return arm_ok[i] != 0; };
@@ -1118,6 +1128,11 @@ int cuda_probe(CudaBackend* be, const b2dp_probe_opts* opts, std::vector<b2dp_pr
             }
         }
         be->gpus[i]->last_healthy = o.healthy;
+    }
+    if (be->cfg.sm_check_ms) {  // after every HBM verdict, before the latches below are merged into this result
+        std::vector<char> ran(n, 0);
+        for (size_t i = 0; i < n; ++i) ran[i] = state[i] == 1 && out[i].err == B2DP_OK;
+        sm_check_slices(be, ran, out);
     }
     if (be->cfg.check_xid) {  // opt-in: a critical Xid since open fails the device whatever the pass said
         for (size_t i = 0; i < n; ++i)
@@ -2303,6 +2318,63 @@ static int cuda_sm_test(CudaBackend* be, int suite, int device, const b2dp_compu
                         std::vector<b2dp_compute_test_result>& out, std::string& err) {
     if (suite < 0 || suite >= kSmTests) { err = "unknown SM self-test"; return B2DP_E_INVAL; }
     return cuda_diag_test(*kSuites[suite], kSmTestNames[suite], be, device, opts, out, err);
+}
+
+// ---- sm_check=: one SM self-test slice per probe pass, in rotation ---------------------------------------------------
+// cuda_probe calls this under probe_mu, after every HBM verdict of the pass (whose fields it leaves as they are) and
+// before the latches are merged into the results, with ran[i] set for each GPU whose pass completed in this call.  Each
+// of those GPUs that no other process uses runs the next suite of its own rotation, kSuites[g->sm_check_next], through
+// compute_test_one on its worker -- all GPUs at once -- for sm_check_ms per format, with a fresh seed and the on-demand
+// tests' default timeout.  A GPU moves on to the next suite only when it ran one, so each runs all kSmTests suites
+// once every kSmTests of its idle passes.  A failed or timed-out slice sets the on-demand tests' latch, which the same
+// result then reports; no health event is fired, because the beat that ran the slice already carries the verdict.
+static void sm_check_slices(CudaBackend* be, const std::vector<char>& ran, std::vector<b2dp_probe_result>& out) {
+    const uint32_t duration_ms = be->cfg.sm_check_ms, timeout_ms = 10000u + 6u * duration_ms;
+    b2dp_compute_test_opts o{};
+    o.duration_ms = duration_ms;
+    o.timeout_ms = timeout_ms;
+    o.fault_sm = be->cfg.sm_check_fault_sm;
+    o.fault_mask = be->cfg.sm_check_fault_mask;
+    const uint32_t seed = (uint32_t)std::chrono::steady_clock::now().time_since_epoch().count() * kPatternMul;
+    const size_t n = be->gpus.size();
+    std::vector<b2dp_compute_test_result> res(n);
+    std::vector<std::string> errs(n);
+    std::vector<double> wall_ms(n, 0.0);
+    std::vector<std::shared_ptr<Completion>> cs(n);
+    for (size_t i = 0; i < n; ++i) {
+        Gpu* g = be->gpus[i].get();
+        if (!ran[i] || used_by_another_process(be, g)) continue;  // a tenant's kernels never share SMs with a slice
+        const DiagSuite* su = kSuites[g->sm_check_next];
+        b2dp_compute_test_result* r = &res[i];
+        r->device = (int32_t)i;
+        r->seed = su->per_device_seed ? seed ^ ((uint32_t)i << 16) : seed;
+        r->sm_count = (int32_t)g->sms;
+        r->first_bad_sm = r->first_bad_format = r->first_bad_tile = -1;
+        std::string* e = &errs[i];
+        double* wall = &wall_ms[i];
+        cs[i] = post(g, [su, be, g, o, duration_ms, timeout_ms, r, e, wall] {
+            const auto t0 = std::chrono::steady_clock::now();
+            compute_test_one(*su, be, g, o, duration_ms, timeout_ms, nullptr, r, e);  // builds its tables here
+            *wall = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+        });
+    }
+    for (size_t i = 0; i < n; ++i) {
+        if (!cs[i]) continue;
+        cs[i]->wait();  // no deadline here: the buffers must be released before the pass returns
+        Gpu* g = be->gpus[i].get();
+        const int k = g->sm_check_next;
+        g->sm_check_next = (k + 1) % kSmTests;
+        const b2dp_compute_test_result& r = res[i];
+        out[i].flags |= B2DP_RES_SM_CHECK;
+        out[i].sm_check = (uint32_t)(k + 1);
+        if (!r.healthy) g->compute_fault.store(true);
+        logf(r.healthy ? 0 : 2, "%s SM check %s: %s, SMs %d/%d, mismatches %s %llu/%llu/%llu, %.1f/%.1f/%.1f ms, "
+             "%.1f ms on the worker%s%s%s", g->dev.id.c_str(), kSuites[k]->log_name,
+             r.healthy ? "Healthy" : "Unhealthy (latched)", r.sms_covered, r.sm_count, kSuites[k]->format_names,
+             (unsigned long long)r.mismatches[0], (unsigned long long)r.mismatches[1],
+             (unsigned long long)r.mismatches[2], r.ms[0], r.ms[1], r.ms[2], wall_ms[i],
+             r.err == B2DP_E_TIMEOUT ? ", timed out" : "", errs[i].empty() ? "" : ", ", errs[i].c_str());
+    }
 }
 
 // ---- on-demand host-link self-test (b2dp_hostlink_test) ---------------------------------------------------------------

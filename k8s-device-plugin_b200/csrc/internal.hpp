@@ -119,6 +119,9 @@ struct CudaConfig {
     bool check_ecc = false;
     bool check_xid = false;
     std::vector<int> break_devices;      // test hook: indices (enumeration order) whose per-GPU setup is treated as failed
+    uint32_t sm_check_ms = 0;            // sm_check=: ms per format of the SM self-test slice after every pass (0 = off)
+    int sm_check_fault_sm = -1;          // sm_check_fault=<smid>+<mask>: test hook handed to every slice
+    uint32_t sm_check_fault_mask = 0;
 };
 int cuda_backend_open(const CudaConfig& cfg, CudaBackend** out, std::string& err);
 void cuda_backend_close(CudaBackend*);
